@@ -181,6 +181,35 @@ int svo_b200_sia_config(svo_b200_ctx* ctx, int ctas_per_pair, int features_per_t
  * svo/src/sparse_img_align.cpp:84-145 runs it lazily per level).  mode: -1 = automatic (default), 0 = per level, 1 = as -1. */
 int svo_b200_sia_upfront(svo_b200_ctx* ctx, int mode);
 
+/* How the current image of one pyramid level reaches the alignment kernel's residual loop. */
+#define SVO_B200_SIA_STAGE_GLOBAL 0 /* gathered from global memory */
+#define SVO_B200_SIA_STAGE_IMAGE 1  /* the whole level copied into shared memory by one TMA bulk copy */
+#define SVO_B200_SIA_STAGE_WINDOW 2 /* a 16x8-byte window per feature copied into shared memory with cp.async */
+/* The launch of the most recent svo_b200_sparse_img_align, svo_b200_sparse_residuals or svo_b200_sia_batch_run:
+ * which kernel instantiation ran and how it staged every level (tests and tuning). */
+typedef struct {
+  int n_pairs;             /* B */
+  int ctas_per_pair;       /* 1, or the thread-block cluster size 2, 4, 8 */
+  int threads;             /* per CTA */
+  int features_per_thread; /* 1 or 2 */
+  int min_blocks;          /* resident CTAs per SM the instantiation is compiled for (__launch_bounds__) */
+  int upfront;             /* cluster geometry with all levels prepared before the first iteration */
+  int async_exchange;      /* upfront variant exchanging the per-iteration sums by st.async + mbarrier */
+  int patch_cache;         /* throughput geometry with the 128-byte patch cache (SVO_B200_SIA_BQ=1) */
+  int general_camera;      /* 1 = general camera models compiled in, 0 = the undistorted-pinhole instantiation */
+  int residuals_only;      /* 1 = the svo_b200_sparse_residuals pass */
+  int prefetch;            /* the next level's staged image is prefetched into L2 (SVO_B200_SIA_PREFETCH) */
+  int stage_cap;           /* bytes of the shared-memory staging region */
+  int smem_bytes;          /* dynamic shared memory per CTA */
+  int resident_clusters;   /* cudaOccupancyMaxActiveClusters of the 4-CTA upfront cluster kernel as the choice last consulted
+                              it (0 = not consulted by this context yet) */
+  int sm_count;            /* multiprocessors of the device */
+  int min_level, max_level;
+  int level_stage[SVO_B200_MAX_LEVELS]; /* SVO_B200_SIA_STAGE_* of levels min_level..max_level, -1 elsewhere */
+} svo_b200_sia_launch;
+/* Returns SVO_B200_EINVAL if the context has not launched the alignment kernel yet. */
+int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out);
+
 /* ---- one stream's features split over several GPUs (SURVEY.md 8e; a demonstration mode: a pair fits one GPU) ----
  * Every rank (one process or thread per GPU) holds both pyramids and passes ITS contiguous slice of the pair's features
  * to svo_b200_sparse_img_align / svo_b200_sia_batch_*; the kernels of the ranks exchange the per-iteration sums

@@ -39,6 +39,16 @@ class SiaStats(C.Structure):
                 ("n_tracked", C.c_int32)]
 
 
+SIA_STAGE_NAMES = {-1: None, 0: "global", 1: "image", 2: "window"}  # SVO_B200_SIA_STAGE_*
+
+
+class SiaLaunch(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("n_pairs", "ctas_per_pair", "threads", "features_per_thread", "min_blocks", "upfront",
+                                       "async_exchange", "patch_cache", "general_camera", "residuals_only", "prefetch", "stage_cap",
+                                       "smem_bytes", "resident_clusters", "sm_count", "min_level", "max_level")] + \
+                [("level_stage", C.c_int * MAX_LEVELS)]
+
+
 class MatchOptions(C.Structure):
     _fields_ = [("max_search_level", C.c_int), ("align_max_iter", C.c_int)]
 
@@ -307,6 +317,15 @@ class Context:
     def sia_config(self, ctas_per_pair=-1, features_per_thread=0):
         """Launch geometry of the alignment kernel (svo_b200_sia_config): -1 / 0 = automatic."""
         self._check(self.lib.svo_b200_sia_config(self.h, int(ctas_per_pair), int(features_per_thread)))
+
+    def sia_last_launch(self) -> dict:
+        """The launch of the most recent alignment / residual / batch call (svo_b200_sia_last_launch): the instantiation's
+        parameters, with `stages` = {level: "global" | "image" | "window"} for the levels it ran."""
+        L = SiaLaunch()
+        self._check(self.lib.svo_b200_sia_last_launch(self.h, C.byref(L)))
+        d = {name: getattr(L, name) for name, _ in SiaLaunch._fields_ if name != "level_stage"}
+        d["stages"] = {lv: SIA_STAGE_NAMES[L.level_stage[lv]] for lv in range(L.min_level, L.max_level + 1)}
+        return d
 
     def sia_batch_run(self):
         self._check(self.lib.svo_b200_sia_batch_run(self.h))

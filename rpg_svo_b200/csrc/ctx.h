@@ -70,6 +70,8 @@ struct svo_b200_ctx {
   // cudaOccupancyMaxActiveClusters of the 4-CTA cluster kernel ([0] upfront, [1] per level) at the shared memory it was asked for
   size_t sia_occ_smem[2] = {0, 0};
   int sia_occ_clusters[2] = {0, 0};
+  svo_b200_sia_launch sia_last = {};  // svo_b200_sia_last_launch
+  bool sia_last_valid = false;
 };
 
 namespace svo {

@@ -535,6 +535,20 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) 
 }
 
 enum { kModeGlobal = 0, kModeImage = 1, kModeWindow = 2 };
+static_assert(kModeGlobal == SVO_B200_SIA_STAGE_GLOBAL && kModeImage == SVO_B200_SIA_STAGE_IMAGE && kModeWindow == SVO_B200_SIA_STAGE_WINDOW,
+              "the staging modes are reported through the ABI");
+
+// How the current image of a W x Hh level reaches the residual loop: whole by one TMA copy when it fits the staging region
+// (with 16 bytes to spare: the aligned-word fetches read past the last pixel), else -- in instantiations that have windows
+// (`win`) -- one window per feature slot when the rows are 8-byte aligned and `slots` windows fit, else gathers from global
+// memory.  The kernel and svo_b200_sia_last_launch both decide with this function.
+__host__ __device__ __forceinline__ uint32_t sia_image_bytes(int W, int Hh) { return ((uint32_t)(W * Hh) + 15u) & ~15u; }
+__host__ __device__ __forceinline__ int sia_stage_mode(uint32_t img_bytes, int W, int stage_cap, bool win, int use_windows, int slots) {
+  int mode = kModeGlobal;
+  if (img_bytes + 16u <= (uint32_t)stage_cap) mode = kModeImage;
+  else if (win && use_windows && (W & 7) == 0 && kWinBytes * slots <= stage_cap) mode = kModeWindow;
+  return mode;
+}
 
 // slot of Bq[r][c] in the 32-value patch cache (BQ): row 0 cols 1..4 -> 0..3, rows 1..4 cols 0..5 -> 4..27, row 5 cols 1..4 -> 28..31
 __host__ __device__ constexpr int bq_idx(int r, int c) { return r == 0 ? c - 1 : r == 5 ? 28 + c - 1 : 4 + (r - 1) * 6 + c; }
@@ -589,20 +603,30 @@ __device__ __forceinline__ void sia_world2cam(const CamDev& c, double x, double 
 //
 // UP = true (cluster geometry, every CTA alone on its SM): patches / H / factorisations of all levels are computed before
 // the first iteration (SiaUpT); shared memory then holds one patch array set per level.
+// Compile-time layout of one instantiation (explained where the kernel uses it); the host reports launches with it.
+template <int FPT, int MAXT, int MINB, int CS>
+struct SiaLayout {
+  static constexpr bool SS = (FPT == 2 && MAXT == 160 && CS == 1);
+  static constexpr int SA = SS ? 304 : MAXT * FPT;
+  static constexpr bool BQ = SS && MINB == 4;
+  static constexpr bool WIN = !SS;
+};
+
 template <int FPT, bool EVAL, int MAXT, int MINB, int CS, bool CG, bool UP>
 __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   static_assert(!UP || (CS > 1 && FPT == 1 && !EVAL), "the upfront variant exists for the cluster geometry only");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using SH = SiaSharedT<MAXT / 32, CS>;
   using UPT = SiaUpT<MAXT / 32, CS>;
+  using LAY = SiaLayout<FPT, MAXT, MINB, CS>;
   SH& s = *reinterpret_cast<SH*>(smem_raw);
   constexpr int S = MAXT * FPT;  // feature slots of this CTA (== P.slots, checked on the host)
   // Throughput geometry (160 threads x 2 features, three CTAs per SM): the shared arrays are allocated for SA = 304 slots
   // (the host selects it for <= 304 features only), which leaves room for the per-feature state xyz_ref in shared memory
   // next to the two coarsest current images.  Kept in registers that state was spilled at 128 registers per thread, and local
   // memory misses the small L1 left beside 3 x 75 KB of shared memory (each miss at the head of a feature's projection chain).
-  constexpr bool SS = (FPT == 2 && MAXT == 160 && CS == 1);
-  constexpr int SA = SS ? 304 : S;  // stride of the per-slot shared arrays
+  constexpr bool SS = LAY::SS;
+  constexpr int SA = LAY::SA;  // stride of the per-slot shared arrays
   // The throughput geometry has no room for windows (its staging region holds the two coarsest current images) and is never
   // used for the multi-GPU feature split: both code paths are compiled out of it, and its residual pass loops over the
   // thread's features instead of being unrolled -- the instruction stream of one Gauss-Newton iteration shrinks from ~27 KB to
@@ -612,9 +636,9 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   // instead of 16 values + 16 gradient pairs -- 128 instead of 192 bytes per feature; dx = (Bq[y][x+1] - Bq[y][x-1]) / 2 and
   // dy likewise are formed in the residual pass with the same two roundings precomputeReferencePatches uses.  That brings a
   // CTA to ~55 KB of shared memory: four pairs per SM instead of three interleave their serial phases.
-  constexpr bool BQ = SS && MINB == 4;
+  constexpr bool BQ = LAY::BQ;
   constexpr int kPatFloats = BQ ? 32 : 3 * kPatchArea;  // floats per feature slot in one patch array set
-  constexpr bool WIN = !SS;  // per-feature cp.async windows of the current image exist in this instantiation
+  constexpr bool WIN = LAY::WIN;  // per-feature cp.async windows of the current image exist in this instantiation
   constexpr bool XG = (CS == 1) && !SS;  // multi-GPU feature split (svo_b200_sia_split_*) compiled in
   constexpr size_t kCtlBytes = ((sizeof(SH) + 15) & ~size_t(15)) + (UP ? ((sizeof(UPT) + 15) & ~size_t(15)) : 0);
   UPT& up = *reinterpret_cast<UPT*>(smem_raw + ((sizeof(SH) + 15) & ~size_t(15)));  // only touched when UP
@@ -978,10 +1002,8 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     const uint8_t* cur_img = job.cur_lvl[level];
 
     // ---- how the current image of this level reaches the residual loop --------------------------
-    const uint32_t img_bytes = ((uint32_t)(W * Hh) + 15u) & ~15u;
-    int mode = kModeGlobal;
-    if (img_bytes + 16u <= (uint32_t)P.stage_cap) mode = kModeImage;
-    else if (WIN && P.use_windows && (W & 7) == 0 && kWinBytes * SA <= P.stage_cap) mode = kModeWindow;
+    const uint32_t img_bytes = sia_image_bytes(W, Hh);
+    int mode = sia_stage_mode(img_bytes, W, P.stage_cap, WIN, P.use_windows, SA);
     // Phase parity of this use of s.mbar, kept by every thread in a register (use k completes parity k & 1; the blob copy was
     // use 0).  NOT read from shared memory: in the upfront variant no barrier separates thread 0's update from the other
     // warps' wait, and a stale parity lets them through before the image has landed (found by running the tests under
@@ -1609,9 +1631,19 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& t
   return 0;
 }
 
+// The template arguments of one sia_kernel instantiation (EVAL is launch_sia's), as a type launch_sia can report.
+template <int FPT_, int MAXT_, int MINB_, int CS_, bool CG_, bool UP_>
+struct SiaInst {
+  static constexpr int FPT = FPT_, MAXT = MAXT_, MINB = MINB_, CS = CS_;
+  static constexpr bool CG = CG_, UP = UP_;
+};
+
 template <bool EVAL>
 static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads, int fpt, int cluster, bool upfront, bool bq, size_t smem) {
-  auto go = [&](auto kern) -> int {
+  auto go = [&](auto inst) -> int {
+    using I = decltype(inst);
+    using LAY = SiaLayout<I::FPT, I::MAXT, I::MINB, I::CS>;
+    const auto kern = sia_kernel<I::FPT, EVAL, I::MAXT, I::MINB, I::CS, I::CG, I::UP>;
     SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // ask for the full shared-memory carveout so that two CTAs of ~95 KB fit one SM
     SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -1633,28 +1665,39 @@ static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads,
     kt_end(ctx);
     ctx->launches++;
     SVO_CUDA_CHECK(ctx, cudaGetLastError());
+    svo_b200_sia_launch& L = ctx->sia_last;  // what ran, for svo_b200_sia_last_launch
+    L = svo_b200_sia_launch{};
+    L.n_pairs = B; L.ctas_per_pair = I::CS; L.threads = threads; L.features_per_thread = I::FPT; L.min_blocks = I::MINB;
+    L.upfront = I::UP; L.async_exchange = I::UP && P.async_xchg; L.patch_cache = LAY::BQ; L.general_camera = I::CG;
+    L.residuals_only = EVAL; L.prefetch = P.use_prefetch; L.stage_cap = P.stage_cap; L.smem_bytes = (int)smem; L.resident_clusters = ctx->sia_occ_clusters[0];
+    L.sm_count = ctx->sm_count;
+    L.min_level = EVAL ? P.eval_level : P.min_level;
+    L.max_level = EVAL ? P.eval_level : P.max_level;
+    for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l)
+      L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, LAY::WIN, P.use_windows, LAY::SA) : -1;
+    ctx->sia_last_valid = true;
     return 0;
   };
   // the undistorted pinhole gets its own instantiation of the geometries that carry the throughput / latency figures
   // (the general-camera code also handles it; EVAL and the rarely used geometries are compiled once)
   const bool plain = !EVAL && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE && g_sia_plain;
-  if (cluster == 2) return go(sia_kernel<1, EVAL, 96, 2, 2, true, false>);
+  if (cluster == 2) return go(SiaInst<1, 96, 2, 2, true, false>{});
   if (cluster == 4) {
     if (upfront && !EVAL)
-      return plain ? go(sia_kernel<1, EVAL, 96, 1, 4, EVAL, !EVAL>) : go(sia_kernel<1, EVAL, 96, 1, 4, true, !EVAL>);
-    return plain ? go(sia_kernel<1, EVAL, 96, 2, 4, EVAL, false>) : go(sia_kernel<1, EVAL, 96, 2, 4, true, false>);
+      return plain ? go(SiaInst<1, 96, 1, 4, EVAL, !EVAL>{}) : go(SiaInst<1, 96, 1, 4, true, !EVAL>{});
+    return plain ? go(SiaInst<1, 96, 2, 4, EVAL, false>{}) : go(SiaInst<1, 96, 2, 4, true, false>{});
   }
-  if (cluster == 8) return go(sia_kernel<1, EVAL, 96, 2, 8, true, false>);
+  if (cluster == 8) return go(SiaInst<1, 96, 2, 8, true, false>{});
   // <= 384 threads: cap registers so that two CTAs are resident per SM
   if (fpt == 1) {
-    if (threads <= 320 && g_sia_minb == 3) return go(sia_kernel<1, EVAL, 320, 3, 1, true, false>);
-    if (threads <= 320) return plain ? go(sia_kernel<1, EVAL, 320, 2, 1, EVAL, false>) : go(sia_kernel<1, EVAL, 320, 2, 1, true, false>);
-    if (threads <= 384) return go(sia_kernel<1, EVAL, 384, 2, 1, true, false>);
-    return go(sia_kernel<1, EVAL, 512, 1, 1, true, false>);
+    if (threads <= 320 && g_sia_minb == 3) return go(SiaInst<1, 320, 3, 1, true, false>{});
+    if (threads <= 320) return plain ? go(SiaInst<1, 320, 2, 1, EVAL, false>{}) : go(SiaInst<1, 320, 2, 1, true, false>{});
+    if (threads <= 384) return go(SiaInst<1, 384, 2, 1, true, false>{});
+    return go(SiaInst<1, 512, 1, 1, true, false>{});
   }
-  if (threads == 160 && bq) return plain ? go(sia_kernel<2, EVAL, 160, 4, 1, EVAL, false>) : go(sia_kernel<2, EVAL, 160, 4, 1, true, false>);
-  if (threads == 160) return plain ? go(sia_kernel<2, EVAL, 160, 3, 1, EVAL, false>) : go(sia_kernel<2, EVAL, 160, 3, 1, true, false>);
-  return go(sia_kernel<2, EVAL, 512, 1, 1, true, false>);
+  if (threads == 160 && bq) return plain ? go(SiaInst<2, 160, 4, 1, EVAL, false>{}) : go(SiaInst<2, 160, 4, 1, true, false>{});
+  if (threads == 160) return plain ? go(SiaInst<2, 160, 3, 1, EVAL, false>{}) : go(SiaInst<2, 160, 3, 1, true, false>{});
+  return go(SiaInst<2, 512, 1, 1, true, false>{});
 }
 
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
@@ -1764,6 +1807,13 @@ int svo_b200_sia_upfront(svo_b200_ctx* ctx, int mode) {
   if (!ctx) return SVO_B200_EINVAL;
   if (mode < -1 || mode > 1) return set_err(ctx, SVO_B200_EINVAL, "sia_upfront: mode must be -1, 0 or 1");
   ctx->sia_upfront = mode;
+  return 0;
+}
+
+int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out) {
+  if (!ctx || !out) return SVO_B200_EINVAL;
+  if (!ctx->sia_last_valid) return set_err(const_cast<svo_b200_ctx*>(ctx), SVO_B200_EINVAL, "sia_last_launch: no alignment kernel launched yet");
+  *out = ctx->sia_last;
   return 0;
 }
 

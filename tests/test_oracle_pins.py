@@ -619,3 +619,49 @@ def test_pyramid_rule_reference_source_compiled_here(oracle, size, levels, ref):
             if cur.shape[1] % 16 == 0:
                 assert not np.array_equal(nxt, oracle.half_sample(cur, oracle.PYR_SCALAR))
             cur = nxt
+
+
+# ---- SparseImgAlign at pyramid sizes whose level widths are not multiples of 16 (the GPU geometry tests use these shapes) ---
+@pytest.mark.parametrize("size", [(644, 484), (648, 488)])
+def test_oracle_sparse_img_align_odd_pyramid_equals_reference_source_compiled_here(oracle, size, ref):
+    """svo::SparseImgAlign::run of the compiled reference at 644x484 (level widths 644, 322, 161, 80, 40) and 648x488 (648,
+    324, 162, ...), with features 3-5 px from all four borders and a motion that moves patches out of the current image:
+    the pyramid takes vikit's scalar branch at every level, and the border tests run against odd widths."""
+    from tests.sia_cases import odd_pair
+
+    p = odd_pair(size)
+    r = ref.call("sparse_img_align", p["ref_pyr"][0], p["cur_pyr"][0], p["n_levels"], p["cam"], p["T_ref_w"], p["T_ref_w"],
+                 p["px"], p["f"], p["pos"], p["has_point"], 4, 0, keep=with_patch_digest)
+    o = oracle.sparse_img_align(p["ref_pyr"], p["cur_pyr"], p["cam"], synth.se3_identity(), p["px"], p["f"], p["pos"],
+                                p["has_point"], p["ref_pos"], 4, 0)
+    assert r["n_tracked"] == o["n_tracked"] and np.array_equal(r["visible"], o["visible"])
+    assert np.allclose(r["T_cur_w"], synth.se3_mul(o["T"], p["T_ref_w"]), rtol=0, atol=1e-8)
+    assert np.allclose(r["H"], o["H"], rtol=1e-8, atol=1e-8)
+    q = oracle.sparse_residuals(p["ref_pyr"][0], p["cur_pyr"][0], 0, p["cam"], o["T"], p["px"], p["f"], p["pos"],
+                                p["has_point"], p["ref_pos"])
+    assert np.array_equal(r["ref_patch"], sha256_u8(q["ref_patch"][r["visible"].astype(bool)]))
+    n_vis = int(o["visible"].sum())
+    assert any(t["n_meas"] // 16 < n_vis for t in o["trace"])  # some pass really lost patches at the border
+    assert not o["visible"].all()                                # and some border features are never visible
+
+
+@pytest.mark.parametrize("level", [0, 1, 2, 4])
+@pytest.mark.parametrize("size", [(644, 484), (648, 488)])
+def test_oracle_residual_pass_odd_pyramid_equals_reference(oracle, size, level, ref):
+    """computeResiduals of the compiled reference at the odd pyramid sizes, at the ground-truth motion (patches at the
+    border leave the current image): visibility, patch cache and every |res| bit for bit, chi2, H_, Jres_."""
+    from tests.sia_cases import odd_pair
+
+    p = odd_pair(size)
+    T = p["T_gt"]
+    r = ref.call("sparse_residuals", p["ref_pyr"][0], p["cur_pyr"][0], p["n_levels"], p["cam"], p["T_ref_w"],
+                 synth.se3_mul(T, p["T_ref_w"]), p["px"], p["f"], p["pos"], p["has_point"], level, keep=with_residual_digest)
+    o = oracle.sparse_residuals(p["ref_pyr"][level], p["cur_pyr"][level], level, p["cam"], T, p["px"], p["f"], p["pos"],
+                                p["has_point"], p["ref_pos"])
+    v, m = o["visible"].astype(bool), o["in_image"].astype(bool)
+    assert np.array_equal(r["visible"], o["visible"]) and np.array_equal(r["ref_patch"], sha256_u8(o["ref_patch"][v]))
+    assert r["n_meas"] == o["n_meas"] == 16 * int(m.sum()) and 0 < m.sum()
+    assert np.array_equal(r["abs_res"], sha256_u8(np.abs(o["residuals"][m])))
+    assert abs(r["chi2"] - o["chi2"]) <= 1e-6 * abs(o["chi2"])
+    assert np.allclose(r["H"], o["H"], rtol=1e-12, atol=1e-9 * np.abs(o["H"]).max())
+    assert np.allclose(r["Jres"], o["Jres"], rtol=1e-9, atol=1e-5)
