@@ -193,12 +193,10 @@ typedef struct {
   int threads;             /* per CTA */
   int features_per_thread; /* 1 or 2 */
   int min_blocks;          /* resident CTAs per SM the instantiation is compiled for (__launch_bounds__) */
-  int upfront;             /* cluster geometry with all levels prepared before the first iteration */
-  int async_exchange;      /* upfront variant exchanging the per-iteration sums by st.async + mbarrier */
-  int patch_cache;         /* throughput geometry with the 128-byte patch cache (SVO_B200_SIA_BQ=1) */
+  int upfront;             /* cluster geometry with all levels prepared before the first iteration; it exchanges the
+                              per-iteration sums by st.async + mbarrier instead of DSMEM stores + barrier.cluster */
   int general_camera;      /* 1 = general camera models compiled in, 0 = the undistorted-pinhole instantiation */
   int residuals_only;      /* 1 = the svo_b200_sparse_residuals pass */
-  int prefetch;            /* the next level's staged image is prefetched into L2 (SVO_B200_SIA_PREFETCH) */
   int stage_cap;           /* bytes of the shared-memory staging region */
   int smem_bytes;          /* dynamic shared memory per CTA */
   int resident_clusters;   /* cudaOccupancyMaxActiveClusters of the 4-CTA upfront cluster kernel as the choice last consulted

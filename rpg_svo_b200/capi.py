@@ -44,8 +44,7 @@ SIA_STAGE_NAMES = {-1: None, 0: "global", 1: "image", 2: "window"}  # SVO_B200_S
 
 class SiaLaunch(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("n_pairs", "ctas_per_pair", "threads", "features_per_thread", "min_blocks", "upfront",
-                                       "async_exchange", "patch_cache", "general_camera", "residuals_only", "prefetch", "stage_cap",
-                                       "smem_bytes", "resident_clusters", "sm_count", "min_level", "max_level")] + \
+                                       "general_camera", "residuals_only", "stage_cap", "smem_bytes", "resident_clusters", "sm_count", "min_level", "max_level")] + \
                 [("level_stage", C.c_int * MAX_LEVELS)]
 
 

@@ -101,8 +101,6 @@ struct SiaParams {
   double eps;
   int stage_cap;  // bytes of the staging region in shared memory (TMA image / cp.async windows)
   int slots;      // blockDim * FPT feature slots per CTA (patch arrays are [3][16][slots])
-  int use_windows, use_prefetch;
-  int async_xchg;  // upfront cluster variant: per-iteration sums by st.async + mbarrier instead of DSMEM stores + barrier.cluster
   double* T_out;
   double* H_out;
   uint8_t* visible_out;
@@ -543,18 +541,12 @@ static_assert(kModeGlobal == SVO_B200_SIA_STAGE_GLOBAL && kModeImage == SVO_B200
 // (`win`) -- one window per feature slot when the rows are 8-byte aligned and `slots` windows fit, else gathers from global
 // memory.  The kernel and svo_b200_sia_last_launch both decide with this function.
 __host__ __device__ __forceinline__ uint32_t sia_image_bytes(int W, int Hh) { return ((uint32_t)(W * Hh) + 15u) & ~15u; }
-__host__ __device__ __forceinline__ int sia_stage_mode(uint32_t img_bytes, int W, int stage_cap, bool win, int use_windows, int slots) {
+__host__ __device__ __forceinline__ int sia_stage_mode(uint32_t img_bytes, int W, int stage_cap, bool win, int slots) {
   int mode = kModeGlobal;
   if (img_bytes + 16u <= (uint32_t)stage_cap) mode = kModeImage;
-  else if (win && use_windows && (W & 7) == 0 && kWinBytes * slots <= stage_cap) mode = kModeWindow;
+  else if (win && (W & 7) == 0 && kWinBytes * slots <= stage_cap) mode = kModeWindow;
   return mode;
 }
-
-// slot of Bq[r][c] in the 32-value patch cache (BQ): row 0 cols 1..4 -> 0..3, rows 1..4 cols 0..5 -> 4..27, row 5 cols 1..4 -> 28..31
-__host__ __device__ constexpr int bq_idx(int r, int c) { return r == 0 ? c - 1 : r == 5 ? 28 + c - 1 : 4 + (r - 1) * 6 + c; }
-static_assert(bq_idx(0, 1) == 0 && bq_idx(0, 4) == 3 && bq_idx(1, 0) == 4 && bq_idx(1, 5) == 9 && bq_idx(4, 5) == 27 &&
-                  bq_idx(5, 1) == 28 && bq_idx(5, 4) == 31,
-              "the 32 used entries of the 6x6 bilinear reference array map onto 0..31 without gaps");
 
 // xyz_cur = T_cur_from_ref * xyz_ref.  One CTA per pair (CS == 1): the pose is read from shared memory (s.pub, published by
 // warp 0's Gauss-Newton tail) at the point of use -- six 128-bit shared loads per feature instead of 24 registers that stay
@@ -604,11 +596,10 @@ __device__ __forceinline__ void sia_world2cam(const CamDev& c, double x, double 
 // UP = true (cluster geometry, every CTA alone on its SM): patches / H / factorisations of all levels are computed before
 // the first iteration (SiaUpT); shared memory then holds one patch array set per level.
 // Compile-time layout of one instantiation (explained where the kernel uses it); the host reports launches with it.
-template <int FPT, int MAXT, int MINB, int CS>
+template <int FPT, int MAXT, int CS>
 struct SiaLayout {
   static constexpr bool SS = (FPT == 2 && MAXT == 160 && CS == 1);
   static constexpr int SA = SS ? 304 : MAXT * FPT;
-  static constexpr bool BQ = SS && MINB == 4;
   static constexpr bool WIN = !SS;
 };
 
@@ -618,7 +609,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using SH = SiaSharedT<MAXT / 32, CS>;
   using UPT = SiaUpT<MAXT / 32, CS>;
-  using LAY = SiaLayout<FPT, MAXT, MINB, CS>;
+  using LAY = SiaLayout<FPT, MAXT, CS>;
   SH& s = *reinterpret_cast<SH*>(smem_raw);
   constexpr int S = MAXT * FPT;  // feature slots of this CTA (== P.slots, checked on the host)
   // Throughput geometry (160 threads x 2 features, three CTAs per SM): the shared arrays are allocated for SA = 304 slots
@@ -631,13 +622,6 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   // used for the multi-GPU feature split: both code paths are compiled out of it, and its residual pass loops over the
   // thread's features instead of being unrolled -- the instruction stream of one Gauss-Newton iteration shrinks from ~27 KB to
   // ~20 KB, which matters with three CTAs in different phases sharing one instruction cache.
-  // BQ (throughput geometry compiled for FOUR CTAs per SM): the patch cache holds the 32 values of the bilinear reference
-  // array the patch and both gradients are made of (rows 1..4 x cols 0..5 and cols 1..4 of rows 0 and 5 of the 6x6 array Bq)
-  // instead of 16 values + 16 gradient pairs -- 128 instead of 192 bytes per feature; dx = (Bq[y][x+1] - Bq[y][x-1]) / 2 and
-  // dy likewise are formed in the residual pass with the same two roundings precomputeReferencePatches uses.  That brings a
-  // CTA to ~55 KB of shared memory: four pairs per SM instead of three interleave their serial phases.
-  constexpr bool BQ = LAY::BQ;
-  constexpr int kPatFloats = BQ ? 32 : 3 * kPatchArea;  // floats per feature slot in one patch array set
   constexpr bool WIN = LAY::WIN;  // per-feature cp.async windows of the current image exist in this instantiation
   constexpr bool XG = (CS == 1) && !SS;  // multi-GPU feature split (svo_b200_sia_split_*) compiled in
   constexpr size_t kCtlBytes = ((sizeof(SH) + 15) & ~size_t(15)) + (UP ? ((sizeof(UPT) + 15) & ~size_t(15)) : 0);
@@ -645,11 +629,11 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   const int n_lvl_bufs = UP ? (P.max_level - P.min_level + 1) : 1;  // patch array sets (one per level when UP)
   float* const pat_base = reinterpret_cast<float*>(smem_raw + kCtlBytes);
   // set li (0 = coarsest level) : [16][S] f32 reference patch, then [16][S] float2 gradients
-  auto pat_ref_of = [&](int li) -> float* { return pat_base + (size_t)li * kPatFloats * SA; };
+  auto pat_ref_of = [&](int li) -> float* { return pat_base + (size_t)li * 3 * kPatchArea * SA; };
   auto pat_dxy_of = [&](int li) -> float2* { return reinterpret_cast<float2*>(pat_ref_of(li) + kPatchArea * SA); };
   float* pat_ref = pat_ref_of(0);
   float2* pat_dxy = pat_dxy_of(0);
-  double* const st_xyz = reinterpret_cast<double*>(pat_base + (size_t)n_lvl_bufs * kPatFloats * SA);  // SS: [3][SA] xyz_ref
+  double* const st_xyz = reinterpret_cast<double*>(pat_base + (size_t)n_lvl_bufs * 3 * kPatchArea * SA);  // SS: [3][SA] xyz_ref
   uint8_t* stage = reinterpret_cast<uint8_t*>(st_xyz + (SS ? 3 * SA : 0));  // 16-byte aligned
   uint4* win = reinterpret_cast<uint4*>(stage);                                                      // [kWinRows][S] 16-byte window rows
 
@@ -711,7 +695,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   double fx_[FPT], fy_[FPT], fz_[FPT], fzi_[FPT];
   double fxs[FPT], fys[FPT], fzs[FPT];  // SS: copies that go to shared memory once the staged blob has been consumed
   int wx_[FPT], wy_[FPT];  // origin of the feature's current-image window (kModeWindow)
-  unsigned hp_mask = 0, vis_mask = 0, in_mask = 0, stale_mask = 0;
+  unsigned hp_mask = 0, vis_mask = 0, in_mask = 0;
 #pragma unroll
   for (int k = 0; k < FPT; ++k) {
     const int i = tid + k * T;
@@ -861,7 +845,6 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
 #pragma unroll(SS ? 1 : FPT)
     for (int k = 0; k < FPT; ++k) {
       m_sxx[k] = m_sxy[k] = m_syy[k] = m_cnt[k] = 0.0;
-      stale_mask &= ~(1u << k);
       const int slot = tid + k * T;
       // px is re-read from the pair's blob in global memory (L2) once per level instead of living in registers
       const double2 pxy = slot < n_loc ? __ldg(reinterpret_cast<const double2*>(job.blob) + fbase + slot) : make_double2(-1e6, -1e6);
@@ -905,10 +888,6 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
           load_row(r + 1, pr1);
 #pragma unroll
           for (int c = 0; c < 6; ++c) b2[c] = bilin(wtl, wtr, wbl, wbr, pr0[c], pr0[c + 1], pr1[c], pr1[c + 1]);
-          if constexpr (BQ) {  // b2 is row r of Bq: cache it (corner columns of rows 0 and 5 are never used)
-#pragma unroll
-            for (int c = (r == 0 || r == 5) ? 1 : 0; c < ((r == 0 || r == 5) ? 5 : 6); ++c) pr[bq_idx(r, c) * SA + slot] = b2[c];
-          }
           if (r >= 2) {  // rows b0 (= Bq[y]), b1 (= Bq[y+1]), b2 (= Bq[y+2]) with y = r-2 are complete
             const int y = r - 2;
 #pragma unroll
@@ -917,10 +896,8 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
               const float val = b1[x + 1];
               const float dx = __fmul_rn(0.5f, __fsub_rn(b1[x + 2], b1[x]));
               const float dy = __fmul_rn(0.5f, __fsub_rn(b2[x + 1], b0[x + 1]));
-              if constexpr (!BQ) {
-                pr[p * SA + slot] = val;
-                pd[p * SA + slot] = make_float2(dx, dy);
-              }
+              pr[p * SA + slot] = val;
+              pd[p * SA + slot] = make_float2(dx, dy);
               sxx = fma((double)dx, (double)dx, sxx);
               sxy = fma((double)dx, (double)dy, sxy);
               syy = fma((double)dy, (double)dy, syy);
@@ -936,14 +913,10 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         // visible from a coarser level but failing here: the reference would keep the stale patch
         // and a zeroed Jacobian (jacobian_cache_.setZero() per level, :64).  Unreachable for
         // dyadic pyramids (SURVEY.md quirk 1) but kept bit-faithful.
-        if constexpr (BQ) {
-          stale_mask |= 1u << k;  // the cache keeps the previous level's Bq: stale values, gradients scaled by zero
-        } else {
 #pragma unroll
-          for (int p = 0; p < kPatchArea; ++p) pd[p * SA + slot] = make_float2(0.f, 0.f);
-          if (pr_stale)  // per-level arrays (upfront variant): the stale patch is the previous level's
-            for (int p = 0; p < kPatchArea; ++p) pr[p * SA + slot] = pr_stale[p * SA + slot];
-        }
+        for (int p = 0; p < kPatchArea; ++p) pd[p * SA + slot] = make_float2(0.f, 0.f);
+        if (pr_stale)  // per-level arrays (upfront variant): the stale patch is the previous level's
+          for (int p = 0; p < kPatchArea; ++p) pr[p * SA + slot] = pr_stale[p * SA + slot];
         m_cnt[k] = 1.0;
       }
     }
@@ -1003,7 +976,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
 
     // ---- how the current image of this level reaches the residual loop --------------------------
     const uint32_t img_bytes = sia_image_bytes(W, Hh);
-    int mode = sia_stage_mode(img_bytes, W, P.stage_cap, WIN, P.use_windows, SA);
+    int mode = sia_stage_mode(img_bytes, W, P.stage_cap, WIN, SA);
     // Phase parity of this use of s.mbar, kept by every thread in a register (use k completes parity k & 1; the blob copy was
     // use 0).  NOT read from shared memory: in the upfront variant no barrier separates thread 0's update from the other
     // warps' wait, and a stale parity lets them through before the image has landed (found by running the tests under
@@ -1016,7 +989,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     }
     if (cta_leader) s.st[g & 1u].old_model = s.st[g & 1u].model;  // optimizeGaussNewton: ModelType old_model(model) [EXT]
     // next level: pull its current image (coarse levels, staged whole) into L2 while this level iterates
-    if (P.use_prefetch && tid == 0 && crank == 0 && level > lvl_lo) {
+    if (tid == 0 && crank == 0 && level > lvl_lo) {
       const uint32_t nb = ((uint32_t)(P.w[level - 1] * P.h[level - 1]) + 15u) & ~15u;
       if (nb + 16u <= (uint32_t)P.stage_cap) prefetch_l2_bulk(job.cur_lvl[level - 1], nb);
     }
@@ -1135,51 +1108,24 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         float q0[5], q1[5];
         q0[0] = byte_to_float<0>(lo[0]); q0[1] = byte_to_float<1>(lo[0]); q0[2] = byte_to_float<2>(lo[0]);
         q0[3] = byte_to_float<3>(lo[0]); q0[4] = byte_to_float<0>(hi[0]);
-        // BQ: three rows of the cached bilinear reference array rotate through registers (row yy cols 1..4, rows yy+1 and yy+2)
-        const float ghalf = ((stale_mask >> k) & 1u) ? 0.f : 0.5f;
-        float bprev[4], bmid[6], bnext[6];
-        if constexpr (BQ) {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) bprev[c] = pat_ref[bq_idx(0, c + 1) * SA + slot];
-#pragma unroll
-          for (int c = 0; c < 6; ++c) bmid[c] = pat_ref[bq_idx(1, c) * SA + slot];
-        }
 #pragma unroll
         for (int yy = 0; yy < 4; ++yy) {
           q1[0] = byte_to_float<0>(lo[yy + 1]); q1[1] = byte_to_float<1>(lo[yy + 1]); q1[2] = byte_to_float<2>(lo[yy + 1]);
           q1[3] = byte_to_float<3>(lo[yy + 1]); q1[4] = byte_to_float<0>(hi[yy + 1]);
-          if constexpr (BQ) {
-#pragma unroll
-            for (int c = (yy == 3) ? 1 : 0; c < ((yy == 3) ? 5 : 6); ++c) bnext[c] = pat_ref[bq_idx(yy + 2, c) * SA + slot];
-          }
 #pragma unroll
           for (int xx = 0; xx < 4; ++xx) {
             const int p = yy * 4 + xx;
             const float I = bilin(wtl, wtr, wbl, wbr, q0[xx], q0[xx + 1], q1[xx], q1[xx + 1]);
-            float val, dx, dy;
-            if constexpr (BQ) {
-              val = bmid[xx + 1];
-              dx = __fmul_rn(ghalf, __fsub_rn(bmid[xx + 2], bmid[xx]));          // as precomputeReferencePatches forms them (:121-126)
-              dy = __fmul_rn(ghalf, __fsub_rn(bnext[xx + 1], bprev[xx]));
-            } else {
-              val = pat_ref[p * SA + slot];
-              const float2 gr = pat_dxy[p * SA + slot];
-              dx = gr.x; dy = gr.y;
-            }
+            const float val = pat_ref[p * SA + slot];
+            const float2 gr = pat_dxy[p * SA + slot];
             const float res = __fsub_rn(I, val);
             c2 = fmaf(res, res, c2);  // chi2 += res*res*weight, weight == 1 (:222); order differs from the serial sum anyway
-            gx = fmaf(dx, res, gx);
-            gy = fmaf(dy, res, gy);
+            gx = fmaf(gr.x, res, gx);
+            gy = fmaf(gr.y, res, gy);
             if (EVAL) P.residuals_out[(size_t)(fbase + slot) * kPatchArea + p] = res;
           }
 #pragma unroll
           for (int c = 0; c < 5; ++c) q0[c] = q1[c];
-          if constexpr (BQ) {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) bprev[c] = bmid[c + 1];
-#pragma unroll
-            for (int c = 0; c < 6; ++c) bmid[c] = bnext[c];
-          }
         }
         const double zi = feat_zi(k, z), X = x * zi, Y = y * zi, dgx = (double)gx, dgy = (double)gy;
         acc[0] = fma(-zi, dgx, acc[0]);
@@ -1202,7 +1148,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       if constexpr (CS == 1) {
         if ((lane & 3) == 0) s.part[buf][gw][lane >> 2] = acc[0];
         if (lane == 0) { s.cnt[buf][gw][0] = w_in; s.cnt[buf][gw][1] = w_out; }
-      } else if (UP && P.async_xchg) {
+      } else if constexpr (UP) {
         // every CTA of the cluster receives every warp's partials by st.async: each store completes its 8 bytes on the
         // receiver's mbarrier of this parity, which one local thread arms with the byte count of all warps of the pair; the
         // receiver wakes when the last byte has landed -- one DSMEM hop, no cluster barrier.  (Two barriers: traffic of
@@ -1219,7 +1165,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         }
         mbar_wait(xb, (g >> 1) & 1u);
       } else {
-        // every CTA of the cluster receives every warp's partials (distributed shared memory stores)
+        // per-level cluster flow: every CTA of the cluster receives every warp's partials (distributed shared memory stores)
         if ((lane & 3) == 0) {
 #pragma unroll
           for (int r = 0; r < CS; ++r) st_cluster_f64(&s.part[buf][gw][lane >> 2], (unsigned)r, acc[0]);
@@ -1229,7 +1175,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
           for (int r = 0; r < CS; ++r) st_cluster_v2s32(&s.cnt[buf][gw][0], (unsigned)r, w_in, w_out);
         }
       }
-      if (!(CS > 1 && UP && P.async_xchg)) pair_sync<CS>();  // barrier A: every warp's partial sums are in place
+      if constexpr (!UP) pair_sync<CS>();  // barrier A: every warp's partial sums are in place
       const int nw_pair = nwarps * CS;
       double tot[7];
       int n_in = 0, n_out = 0, done = 0;
@@ -1257,15 +1203,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
           const int slot = tid + k * T;
 #pragma unroll
           for (int p = 0; p < kPatchArea; ++p) {
-            float2 gr;
-            if constexpr (BQ) {
-              const int yy = p >> 2, xx = p & 3;
-              const float gh = ((stale_mask >> k) & 1u) ? 0.f : 0.5f;
-              gr.x = __fmul_rn(gh, __fsub_rn(pat_ref[bq_idx(yy + 1, xx + 2) * SA + slot], pat_ref[bq_idx(yy + 1, xx) * SA + slot]));
-              gr.y = __fmul_rn(gh, __fsub_rn(pat_ref[bq_idx(yy + 2, xx + 1) * SA + slot], pat_ref[bq_idx(yy, xx + 1) * SA + slot]));
-            } else {
-              gr = pat_dxy[p * SA + slot];
-            }
+            const float2 gr = pat_dxy[p * SA + slot];
             const double dx = (double)gr.x, dy = (double)gr.y;
             q_sxx[k] = fma(dx, dx, q_sxx[k]);
             q_sxy[k] = fma(dx, dy, q_sxy[k]);
@@ -1382,7 +1320,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
               for (int p = 0; p < kPatchArea; ++p)
                 P.residuals_out[(size_t)(fbase + i) * kPatchArea + p] = __int_as_float(0x7fc00000);
             for (int p = 0; p < kPatchArea; ++p)
-              P.ref_patch_out[(size_t)(fbase + i) * kPatchArea + p] = BQ ? pat_ref[bq_idx((p >> 2) + 1, (p & 3) + 1) * SA + i] : pat_ref[p * SA + i];
+              P.ref_patch_out[(size_t)(fbase + i) * kPatchArea + p] = pat_ref[p * SA + i];
           }
         }
         break;
@@ -1443,7 +1381,6 @@ struct SiaBatchState {
   size_t o_T = 0, o_H = 0, o_vis = 0, o_stats = 0, out_bytes = 0;
   int threads = 0, fpt = 1, cluster = 1;
   bool upfront = false;  // cluster geometry with all levels prepared before the first iteration (SiaUpT)
-  bool bq = false;       // throughput geometry with the 32-value patch cache, four CTAs per SM
   size_t smem = 0;
   bool staged = false;
 };
@@ -1470,36 +1407,10 @@ void sia_split_free(svo_b200_ctx* ctx) {
   ctx->xg_world = 1; ctx->xg_rank = 0; ctx->xg_pairs = 0; ctx->xg_connected = false;
 }
 
-// tuning knobs, read once from the environment
-static int g_sia_minb = 2;        // SVO_B200_SIA_MINB: resident CTAs per SM the <=320-feature kernel is compiled for
-static int g_sia_stage_kb = 20;   // SVO_B200_SIA_STAGE_KB: minimum staging region (holds level >= 2 of 640x480)
-static int g_sia_windows = 1;     // SVO_B200_SIA_WINDOWS=0: fine levels gather from global memory instead of cp.async windows
-static int g_sia_prefetch = 1;    // SVO_B200_SIA_PREFETCH=0: no bulk L2 prefetch of the next (coarse, TMA-staged) current image.
-                                  // (No per-feature L2 prefetches of the next level's footprints: the extra
-                                  // uncoalesced requests cost more L1 time than the DRAM latency they hide.)
-static int g_sia_cluster = -1;    // SVO_B200_SIA_CLUSTER: force the CTAs per pair (1, 2, 4, 8); -1 = by batch size
-static int g_sia_upfront = 1;     // SVO_B200_SIA_UPFRONT=0: the cluster geometry prepares each level when it reaches it (round-2a behaviour)
-static int g_sia_bq = 0;          // SVO_B200_SIA_BQ=1: throughput geometry with the 128-byte patch cache at four CTAs per SM
-static int g_sia_async = 1;       // SVO_B200_SIA_ASYNC=0: the upfront variant exchanges its sums through barrier.cluster like the others
-static int g_sia_plain = 1;       // SVO_B200_SIA_PLAIN=0: the undistorted pinhole runs the general-camera instantiation too
-static int g_sia_fpt2 = 1;        // SVO_B200_SIA_FPT2: <= 320 features per CTA as 160 threads x 2 features: 1 = three CTAs per SM (default,
-                                  // for full batches), 2 = two CTAs per SM with windows, 0 = 320 threads x 1 feature
-
-static void read_env_once() {
-  static bool env_read = false;
-  if (env_read) return;
-  env_read = true;
-  if (const char* e = getenv("SVO_B200_SIA_MINB")) g_sia_minb = atoi(e) == 3 ? 3 : 2;
-  if (const char* e = getenv("SVO_B200_SIA_STAGE_KB")) g_sia_stage_kb = atoi(e) > 0 ? atoi(e) : 20;
-  if (const char* e = getenv("SVO_B200_SIA_WINDOWS")) g_sia_windows = atoi(e) != 0;
-  if (const char* e = getenv("SVO_B200_SIA_PREFETCH")) g_sia_prefetch = atoi(e) != 0;
-  if (const char* e = getenv("SVO_B200_SIA_CLUSTER")) g_sia_cluster = atoi(e);
-  if (const char* e = getenv("SVO_B200_SIA_FPT2")) g_sia_fpt2 = atoi(e);
-  if (const char* e = getenv("SVO_B200_SIA_PLAIN")) g_sia_plain = atoi(e) != 0;
-  if (const char* e = getenv("SVO_B200_SIA_UPFRONT")) g_sia_upfront = atoi(e) != 0;
-  if (const char* e = getenv("SVO_B200_SIA_ASYNC")) g_sia_async = atoi(e) != 0;
-  if (const char* e = getenv("SVO_B200_SIA_BQ")) g_sia_bq = atoi(e) != 0;
-}
+// Minimum staging region: holds the current image of level >= 2 of 640x480 (TMA).  The next coarse, TMA-staged current
+// image is bulk-prefetched into L2 while a level iterates; there are no per-feature L2 prefetches of the next level's
+// footprints: the extra uncoalesced requests cost more L1 time than the DRAM latency they hide.
+constexpr size_t kSiaMinStageBytes = 20 * 1024;
 
 // Launch geometry for a batch of B pairs with at most max_feat features each.
 //   cluster == 1: one CTA per pair, 320 / 384 / 512 threads (one feature per thread up to 512, two up to 1024);
@@ -1552,12 +1463,11 @@ static int max_active_clusters(svo_b200_ctx* ctx, bool upfront, size_t smem, int
 
 // `fallback` (internal): 1 = the upfront clusters of this batch are not all resident at once, 2 = no cluster geometry is.
 static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& threads, int& fpt, int& cluster, bool& upfront,
-                       bool& bq, int& stage_cap, size_t& smem, int fallback = 0) {
-  read_env_once();
+                       int& stage_cap, size_t& smem, int fallback = 0) {
   if (max_feat > 1024)
     return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features per pair > 1024 (shared-memory patch cache)", max_feat);
   cluster = 1;
-  int want = ctx->sia_cluster >= 0 ? ctx->sia_cluster : g_sia_cluster;
+  int want = ctx->sia_cluster;
   const bool auto_cluster = want < 0 && !ctx->xg_connected;
   if (ctx->xg_connected) {
     // feature split over GPUs: the ranks' CTAs of a pair wait for each other, so every CTA must be resident at once
@@ -1570,10 +1480,9 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& t
   // still has an SM of its own (two cluster CTAs sharing an SM lose to one 320-thread CTA per pair)
   if (want < 0) want = (fallback < 2 && B * 4 <= ctx->sm_count) ? 4 : 1;
   // full batches (more pairs than 2 per SM): 160 threads x 2 features, three CTAs per SM; in between, 320 x 1 with windows
-  int fpt2 = ctx->sia_fpt > 0 ? (ctx->sia_fpt == 2 ? 1 : 0) : g_sia_fpt2;
   // (with its state in shared memory and its loops rolled the 160 x 2 geometry also serves batches below two CTAs per SM,
   // so the 320 x 1 geometry is left for > 304 features per pair, the multi-GPU split and explicit requests)
-  if (ctx->xg_connected) fpt2 = 0;
+  const bool fpt2 = ctx->sia_fpt != 1 && !ctx->xg_connected;
   if (want > 1 && max_feat <= 96 * want && (want == 2 || want == 4 || want == 8)) cluster = want;
   if (cluster > 1) {
     fpt = 1;
@@ -1587,35 +1496,33 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& t
     if (fpt2 && max_feat <= 304) { fpt = 2; threads = 160; }  // its shared arrays are allocated for 304 slots (kernel: SA)
   }
   const bool throughput_geom = cluster == 1 && fpt == 2 && threads == 160;
-  bq = throughput_geom && g_sia_bq && fpt2 != 2;
   const int slots = throughput_geom ? 304 : threads * fpt;
-  size_t base = ((sia_shared_bytes(threads, cluster) + 15) & ~size_t(15)) + (size_t)(bq ? 32 : 3 * kPatchArea) * slots * sizeof(float);
+  size_t base = ((sia_shared_bytes(threads, cluster) + 15) & ~size_t(15)) + (size_t)3 * kPatchArea * slots * sizeof(float);
   if (throughput_geom) base += (size_t)3 * slots * sizeof(double);  // xyz_ref of every feature (kernel: st_xyz)
   // cluster geometry with every CTA alone on its SM: one patch array set per level, everything pose independent prepared
   // before the first iteration (the launch asks for the 4-CTA instantiation; 2 and 8 keep the per-level flow)
   upfront = false;
-  if (cluster == 4 && g_sia_upfront && ctx->sia_upfront != 0 && fallback == 0 && B * cluster <= ctx->sm_count && n_lvl >= 1 &&
+  if (cluster == 4 && ctx->sia_upfront != 0 && fallback == 0 && B * cluster <= ctx->sm_count && n_lvl >= 1 &&
       n_lvl <= SVO_B200_MAX_LEVELS) {
     const size_t base_up = ((sia_shared_bytes(threads, cluster) + 15) & ~size_t(15)) + ((sia_upfront_bytes(cluster) + 15) & ~size_t(15)) +
                            (size_t)n_lvl * 3 * kPatchArea * slots * sizeof(float);
-    if (base_up + (size_t)g_sia_stage_kb * 1024 + 1024 <= (size_t)ctx->max_smem_optin) {
+    if (base_up + kSiaMinStageBytes + 1024 <= (size_t)ctx->max_smem_optin) {
       upfront = true;
       base = base_up;
     }
   }
   // shared memory one CTA may use so that the intended number of CTAs stays resident per SM (228 KB per SM, 1 KB
   // reserved per CTA)
-  const int resident = upfront ? 1 : cluster > 1 ? 2 : (threads == 160 ? (bq ? 4 : fpt2 == 2 ? 2 : 3) : threads <= 384 ? 2 : 1);
+  const int resident = upfront ? 1 : cluster > 1 ? 2 : threads == 160 ? 3 : threads <= 384 ? 2 : 1;
   size_t budget = (size_t)ctx->max_smem_optin;
   const size_t per_cta = (size_t)(228 * 1024) / resident - 1024;
   if (per_cta < budget) budget = per_cta;
   if (base + 1024 > budget)
     return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features need %zu B of shared memory", max_feat, base);
-  // staging region: the coarse current-level images (TMA; 20 KB holds level >= 2 of 640x480) or, at the fine levels,
-  // one 96-byte window per feature slot
-  size_t cap = (size_t)g_sia_stage_kb * 1024;
+  // staging region: the coarse current-level images (TMA) or, at the fine levels, one 128-byte window per feature slot
+  size_t cap = kSiaMinStageBytes;
   const size_t win = (size_t)kWinBytes * slots;
-  if (g_sia_windows && win > cap && base + win <= budget) cap = win;
+  if (win > cap && base + win <= budget) cap = win;
   if (base + cap > budget) cap = (budget - base) & ~size_t(15);
   stage_cap = (int)cap;
   smem = base + cap;
@@ -1626,7 +1533,7 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& t
   if (auto_cluster && cluster == 4 && !(upfront && ctx->sia_upfront == 1)) {
     int n = 0;
     if (int rc = max_active_clusters(ctx, upfront, smem, n)) return rc;
-    if (B > n) return pick_launch(ctx, B, max_feat, n_lvl, threads, fpt, cluster, upfront, bq, stage_cap, smem, upfront ? 1 : 2);
+    if (B > n) return pick_launch(ctx, B, max_feat, n_lvl, threads, fpt, cluster, upfront, stage_cap, smem, upfront ? 1 : 2);
   }
   return 0;
 }
@@ -1639,10 +1546,10 @@ struct SiaInst {
 };
 
 template <bool EVAL>
-static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads, int fpt, int cluster, bool upfront, bool bq, size_t smem) {
+static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads, int fpt, int cluster, bool upfront, size_t smem) {
   auto go = [&](auto inst) -> int {
     using I = decltype(inst);
-    using LAY = SiaLayout<I::FPT, I::MAXT, I::MINB, I::CS>;
+    using LAY = SiaLayout<I::FPT, I::MAXT, I::CS>;
     const auto kern = sia_kernel<I::FPT, EVAL, I::MAXT, I::MINB, I::CS, I::CG, I::UP>;
     SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // ask for the full shared-memory carveout so that two CTAs of ~95 KB fit one SM
@@ -1668,34 +1575,34 @@ static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads,
     svo_b200_sia_launch& L = ctx->sia_last;  // what ran, for svo_b200_sia_last_launch
     L = svo_b200_sia_launch{};
     L.n_pairs = B; L.ctas_per_pair = I::CS; L.threads = threads; L.features_per_thread = I::FPT; L.min_blocks = I::MINB;
-    L.upfront = I::UP; L.async_exchange = I::UP && P.async_xchg; L.patch_cache = LAY::BQ; L.general_camera = I::CG;
-    L.residuals_only = EVAL; L.prefetch = P.use_prefetch; L.stage_cap = P.stage_cap; L.smem_bytes = (int)smem; L.resident_clusters = ctx->sia_occ_clusters[0];
+    L.upfront = I::UP; L.general_camera = I::CG;
+    L.residuals_only = EVAL; L.stage_cap = P.stage_cap; L.smem_bytes = (int)smem; L.resident_clusters = ctx->sia_occ_clusters[0];
     L.sm_count = ctx->sm_count;
     L.min_level = EVAL ? P.eval_level : P.min_level;
     L.max_level = EVAL ? P.eval_level : P.max_level;
     for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l)
-      L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, LAY::WIN, P.use_windows, LAY::SA) : -1;
+      L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, LAY::WIN, LAY::SA) : -1;
     ctx->sia_last_valid = true;
     return 0;
   };
   // the undistorted pinhole gets its own instantiation of the geometries that carry the throughput / latency figures
-  // (the general-camera code also handles it; EVAL and the rarely used geometries are compiled once)
-  const bool plain = !EVAL && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE && g_sia_plain;
+  // (the general-camera code also handles it; EVAL and the rarely used geometries are compiled once: with EVAL, CG = EVAL
+  // names the general-camera instantiation in both arms)
+  const bool plain = !EVAL && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE;
   if (cluster == 2) return go(SiaInst<1, 96, 2, 2, true, false>{});
   if (cluster == 4) {
-    if (upfront && !EVAL)
-      return plain ? go(SiaInst<1, 96, 1, 4, EVAL, !EVAL>{}) : go(SiaInst<1, 96, 1, 4, true, !EVAL>{});
+    if constexpr (!EVAL) {
+      if (upfront) return plain ? go(SiaInst<1, 96, 1, 4, false, true>{}) : go(SiaInst<1, 96, 1, 4, true, true>{});
+    }
     return plain ? go(SiaInst<1, 96, 2, 4, EVAL, false>{}) : go(SiaInst<1, 96, 2, 4, true, false>{});
   }
   if (cluster == 8) return go(SiaInst<1, 96, 2, 8, true, false>{});
   // <= 384 threads: cap registers so that two CTAs are resident per SM
   if (fpt == 1) {
-    if (threads <= 320 && g_sia_minb == 3) return go(SiaInst<1, 320, 3, 1, true, false>{});
     if (threads <= 320) return plain ? go(SiaInst<1, 320, 2, 1, EVAL, false>{}) : go(SiaInst<1, 320, 2, 1, true, false>{});
     if (threads <= 384) return go(SiaInst<1, 384, 2, 1, true, false>{});
     return go(SiaInst<1, 512, 1, 1, true, false>{});
   }
-  if (threads == 160 && bq) return plain ? go(SiaInst<2, 160, 4, 1, EVAL, false>{}) : go(SiaInst<2, 160, 4, 1, true, false>{});
   if (threads == 160) return plain ? go(SiaInst<2, 160, 3, 1, EVAL, false>{}) : go(SiaInst<2, 160, 3, 1, true, false>{});
   return go(SiaInst<2, 512, 1, 1, true, false>{});
 }
@@ -1724,10 +1631,6 @@ static int fill_common(svo_b200_ctx* ctx, SiaParams& P, const svo_b200_frame* fr
   if (rc) return rc;
   P.max_level = opt->max_level; P.min_level = opt->min_level; P.n_iter = opt->n_iter; P.eps = opt->eps;
   P.debug = getenv("SVO_B200_SIA_DEBUG") ? 1 : 0;
-  read_env_once();
-  P.use_windows = g_sia_windows;
-  P.use_prefetch = g_sia_prefetch;
-  P.async_xchg = g_sia_async;
   P.xg.rank = 0; P.xg.world = 1;
   if (ctx->xg_connected) {
     P.xg.rank = ctx->xg_rank; P.xg.world = ctx->xg_world;
@@ -1845,7 +1748,7 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
   int rc = fill_common(ctx, st.P, ref[0], cam, opt);
   if (rc) return rc;
   int stage_cap = 0;
-  rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.threads, st.fpt, st.cluster, st.upfront, st.bq,
+  rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.threads, st.fpt, st.cluster, st.upfront,
                    stage_cap, st.smem);
   if (rc) return rc;
   st.P.stage_cap = stage_cap;
@@ -1905,7 +1808,7 @@ int svo_b200_sia_batch_run(svo_b200_ctx* ctx) {
   if (!ctx || !ctx->sia || !ctx->sia->staged) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_run: nothing staged");
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
-  return launch_sia<false>(ctx, st.P, st.B, st.threads, st.fpt, st.cluster, st.upfront, st.bq, st.smem);
+  return launch_sia<false>(ctx, st.P, st.B, st.threads, st.fpt, st.cluster, st.upfront, st.smem);
 }
 
 int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_out, double* H_out,
@@ -2008,7 +1911,7 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
   st.P.Jres_out = reinterpret_cast<double*>(ds + o_j);
   st.P.chi2_out = reinterpret_cast<double*>(ds + o_c);
   st.P.n_meas_out = reinterpret_cast<long long*>(ds + o_n);
-  if ((rc = launch_sia<true>(ctx, st.P, 1, st.threads, st.fpt, st.cluster, false, st.bq, st.smem))) return rc;
+  if ((rc = launch_sia<true>(ctx, st.P, 1, st.threads, st.fpt, st.cluster, false, st.smem))) return rc;
   double Tdummy[12];
   if ((rc = svo_b200_sia_batch_fetch(ctx, Tdummy, visible_io, H_out, nullptr))) return rc;
   if (ref_patch_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(ref_patch_out, ds + o_rp, sizeof(float) * 16 * (size_t)N, cudaMemcpyDeviceToHost));

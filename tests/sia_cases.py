@@ -1,5 +1,5 @@
-"""Inputs and comparisons shared by the alignment-kernel geometry tests (test_sia_geometry_gpu.py, test_sia_knobs_gpu.py and
-its child script sia_knob_child.py, test_oracle_pins.py): feature sets sized to the capacity edges of every launch
+"""Inputs and comparisons shared by the alignment-kernel tests (test_sia_geometry_gpu.py, test_sia_gpu.py,
+test_oracle_pins.py): feature sets sized to the capacity edges of every launch
 geometry, and frame pairs at pyramid sizes whose levels take every staging path of the kernel."""
 import numpy as np
 

@@ -3,10 +3,13 @@
 Tolerances are the ones BASELINE.json's north_star states: 1e-4 on the final SE3 and on per-patch
 residuals, bit-exact visibility masks.
 """
+import functools
+
 import numpy as np
 import pytest
 
 from rpg_svo_b200 import synth
+from tests import sia_cases as sc
 
 pytestmark = pytest.mark.gpu
 
@@ -68,17 +71,40 @@ def test_iteration_trace_matches(ctx, oracle, pair300):
         assert np.allclose(a["T"], b["T"], atol=1e-6)
 
 
-@pytest.mark.parametrize("level", [0, 1, 2, 3, 4])
-def test_residual_pass_matches(ctx, oracle, pair300, level):
-    d = pair300
-    T = synth.se3_exp(np.array([0.004, -0.003, 0.002, 0.001, -0.002, 0.0015]))
+@functools.lru_cache(maxsize=None)
+def _residual_case(case):
+    """(frame pair, pose) of a residual-pass case: the border case (features 3-5 px from every border, patches leaving the
+    image at the motion) and the ATAN camera (general-camera projection) at their true motion."""
+    if case == "border":
+        d = sc.border_pair(5, 640, 480, 300)
+        return d, d["T_gt"]
+    cam = synth.reference_param_camera("atan")
+    d = synth.make_frame_pair(1000, width=cam.width, height=cam.height, n_feat=300, n_levels=5, cam=cam)
+    return d, d["T_cur_ref_gt"]
+
+
+RESIDUAL_CASES = [("pair300", lv) for lv in range(5)] + [("border", 2), ("atan", 1)]
+
+
+@pytest.mark.parametrize("case,level", RESIDUAL_CASES,
+                         ids=[str(lv) if case == "pair300" else f"{case}-{lv}" for case, lv in RESIDUAL_CASES])
+def test_residual_pass_matches(ctx, oracle, pair300, case, level):
+    if case == "pair300":
+        d, T = pair300, synth.se3_exp(np.array([0.004, -0.003, 0.002, 0.001, -0.002, 0.0015]))
+    else:
+        d, T = _residual_case(case)
     ref = ctx.frame(d["ref_pyr"])
     cur = ctx.frame(d["cur_pyr"])
     g = ctx.sparse_residuals(ref, cur, d["cam"], level, T, d["px"], d["f"], d["pos"], d["has_point"], d["ref_pos"])
+    ref.destroy()
+    cur.destroy()
     o = oracle.sparse_residuals(d["ref_pyr"][level], d["cur_pyr"][level], level, d["cam"], T, d["px"],
                                 d["f"], d["pos"], d["has_point"], d["ref_pos"])
     assert np.array_equal(g["visible"], o["visible"])
     assert np.array_equal(g["in_image"], o["in_image"])
+    # The patch rows of features that are not visible hold whatever the kernel's shared memory held: they depend on the
+    # launch geometry's shared-memory layout (the reference leaves those rows of its cv::Mat cache uninitialised too).  So
+    # the patch cache is compared on the visible rows.
     v = o["visible"].astype(bool)
     assert np.array_equal(g["ref_patch"][v], o["ref_patch"][v])  # f32 stage: bit-exact by construction
     m = o["in_image"].astype(bool)
@@ -119,9 +145,10 @@ def _border_case(seed, n_feat, width=640, height=480, trans=0.08, rot_deg=1.5, m
                 ref_pos=synth.se3_inv(T_ref_w)[:, 3].copy(), T_gt=synth.se3_exp(xi))
 
 
-@pytest.mark.parametrize("n_feat", [300, 37])
-def test_patches_leaving_the_image_slow_path(ctx, oracle, n_feat):
-    d = _border_case(5, n_feat)
+@pytest.mark.parametrize("case", ["300", "37", "edges-300"])
+def test_patches_leaving_the_image_slow_path(ctx, oracle, case):
+    # edges-300: a quarter of the features 3-5 px from one of the four borders, four in the bottom-right corner
+    d = _residual_case("border")[0] if case == "edges-300" else _border_case(5, int(case))
     g, o = _run_both(ctx, oracle, d, 4, 0)
     # the case really exercises the per-iteration in-image test: some pass saw fewer patches than are visible
     vis_per_level = {l: 0 for l in range(5)}
