@@ -269,6 +269,11 @@ typedef struct {
   double estimated_scale, error_init, error_final;
   int64_t num_obs;
   int n_iter_done;
+  /* Which 6x6 solves ran, for tests and diagnostics (they sit in what was padding: size and offsets are unchanged).
+   * n_pivoted_solves: Gauss-Newton iterations whose normal matrix failed the unpivoted LDL^T's pivot test
+   * (a pivot <= 1e-13 * max diagonal) and took the pivoted LDL^T; cov_pivoted: 1 if the covariance took the
+   * Gauss-Jordan inverse for the same reason. */
+  int16_t n_pivoted_solves, cov_pivoted;
   double cov[36];
 } svo_b200_pose_opt_result;
 int svo_b200_pose_optimize(svo_b200_ctx* ctx, double reproj_thresh, int n_iter,

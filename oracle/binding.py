@@ -54,7 +54,8 @@ class MatchResult(C.Structure):
 class EpiResult(C.Structure):
     _fields_ = [("success", C.c_int), ("reject", C.c_int), ("search_level", C.c_int),
                 ("n_zmssd_evals", C.c_int), ("n_align_iter", C.c_int), ("epi_length", C.c_double),
-                ("px_cur", C.c_double * 2), ("depth", C.c_double), ("h_inv", C.c_double)]
+                ("px_cur", C.c_double * 2), ("depth", C.c_double), ("h_inv", C.c_double),
+                ("A_cur_ref", C.c_double * 4)]
 
 
 class PoseOptResult(C.Structure):
@@ -309,7 +310,7 @@ def find_epipolar_match_direct(ref_pyr, cur_pyr, cam, T_cur_ref, ref_px, ref_f, 
                                          int(align_1d), C.byref(out))
     return dict(success=bool(out.success), reject=bool(out.reject), search_level=out.search_level,
                 n_zmssd=out.n_zmssd_evals, epi_length=out.epi_length, px_cur=np.array(out.px_cur[:]),
-                depth=out.depth, h_inv=out.h_inv)
+                depth=out.depth, h_inv=out.h_inv, A_cur_ref=np.array(out.A_cur_ref[:]).reshape(2, 2))
 
 
 def update_seed(x, tau2, a, b, mu, z_range, sigma2):
@@ -326,7 +327,7 @@ def compute_tau(T_ref_cur, f, z, px_error_angle):
 
 def depth_filter_update(ref_pyrs, ref_T_f_w, cur_pyr, cur_T_f_w, cam, ref_index, ftr_px, ftr_f,
                         ftr_level, ftr_type, ftr_grad, batch_id, batch_counter, seeds, max_n_kfs=3,
-                        sigma2_thresh=200.0, max_search_level=2):
+                        sigma2_thresh=200.0, max_search_level=2, align_max_iter=10, max_epi_search_steps=1000):
     """seeds: dict of float32 arrays a,b,mu,z_range,sigma2 (updated copies are returned)."""
     n_ref = len(ref_pyrs)
     nl = len(cur_pyr)
@@ -349,7 +350,8 @@ def depth_filter_update(ref_pyrs, ref_T_f_w, cur_pyr, cur_T_f_w, cam, ref_index,
     lib().orc_depth_filter_update(flat, _p(refT), n_ref, cp, _p(c64(cur_T_f_w).reshape(12)), _p(cols),
                                   _p(rows), nl, C.byref(cs), M, _p(ri), _p(fpx), _p(ff), _p(fl),
                                   _p(ft), _p(fg), _p(bi), batch_counter, max_n_kfs,
-                                  C.c_double(sigma2_thresh), max_search_level, _p(out["a"]),
+                                  C.c_double(sigma2_thresh), max_search_level, int(align_max_iter),
+                                  int(max_epi_search_steps), _p(out["a"]),
                                   _p(out["b"]), _p(out["mu"]), _p(out["z_range"]), _p(out["sigma2"]),
                                   _p(status), _p(pxc), _p(z), _p(nz))
     out.update(status=status, px_cur=pxc, z=z, n_zmssd=nz)

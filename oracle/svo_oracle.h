@@ -138,6 +138,7 @@ typedef struct {
   double px_cur[2];
   double depth;
   double h_inv;
+  double A_cur_ref[4]; /* Matcher::A_cur_ref_, row-major */
 } orc_epi_result;
 void orc_find_epipolar_match_direct(const uint8_t* const* ref_levels,
                                     const uint8_t* const* cur_levels, const int* cols,
@@ -171,9 +172,10 @@ void orc_depth_filter_update(
     const int* rows, int n_levels, const orc_camera* cam, int M, const int* ref_index,
     const double* ftr_px, const double* ftr_f, const int* ftr_level, const int* ftr_type,
     const double* ftr_grad, const int* batch_id, int batch_counter, int max_n_kfs,
-    double seed_convergence_sigma2_thresh, int max_search_level, float* a, float* b, float* mu,
-    float* z_range, float* sigma2, uint8_t* status_out, double* px_cur_out /*M*2*/,
-    double* z_out /*M*/, int* n_zmssd_out /*M or NULL*/);
+    double seed_convergence_sigma2_thresh, int max_search_level, int align_max_iter,
+    int max_epi_search_steps, float* a, float* b, float* mu, float* z_range, float* sigma2,
+    uint8_t* status_out, double* px_cur_out /*M*2*/, double* z_out /*M*/,
+    int* n_zmssd_out /*M or NULL*/);
 
 /* ---- pose optimizer (svo/src/pose_optimizer.cpp:28-161) ---- */
 typedef struct {

@@ -54,7 +54,8 @@ class MatchOptions(C.Structure):
 
 class PoseOptResult(C.Structure):
     _fields_ = [("estimated_scale", C.c_double), ("error_init", C.c_double), ("error_final", C.c_double),
-                ("num_obs", C.c_int64), ("n_iter_done", C.c_int), ("cov", C.c_double * 36)]
+                ("num_obs", C.c_int64), ("n_iter_done", C.c_int), ("n_pivoted_solves", C.c_int16),
+                ("cov_pivoted", C.c_int16), ("cov", C.c_double * 36)]
 
 
 class DepthOptions(C.Structure):
@@ -429,7 +430,7 @@ def _pose_optimize(self, reproj_thresh, n_iter, fx, T_f_w, f, pos, level, has_po
                                                 _p(f), _p(pos), _p(lv), _p(hp), len(hp), C.byref(out)))
     return dict(T=T.reshape(3, 4), has_point=hp, estimated_scale=out.estimated_scale, error_init=out.error_init,
                 error_final=out.error_final, num_obs=out.num_obs, n_iter_done=out.n_iter_done,
-                cov=np.array(out.cov[:]).reshape(6, 6))
+                n_pivoted_solves=out.n_pivoted_solves, cov_pivoted=out.cov_pivoted, cov=np.array(out.cov[:]).reshape(6, 6))
 
 
 def _pose_optimize_batch(self, reproj_thresh, n_iter, fx, T_f_w, obs_offset, f, pos, level, has_point):
@@ -447,7 +448,7 @@ def _pose_optimize_batch(self, reproj_thresh, n_iter, fx, T_f_w, obs_offset, f, 
         o = out[b]
         res.append(dict(T=T[b].reshape(3, 4), has_point=hp[off[b]:off[b + 1]], estimated_scale=o.estimated_scale,
                         error_init=o.error_init, error_final=o.error_final, num_obs=o.num_obs, n_iter_done=o.n_iter_done,
-                        cov=np.array(o.cov[:]).reshape(6, 6)))
+                        n_pivoted_solves=o.n_pivoted_solves, cov_pivoted=o.cov_pivoted, cov=np.array(o.cov[:]).reshape(6, 6)))
     return res
 
 

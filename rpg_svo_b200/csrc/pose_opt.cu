@@ -62,7 +62,7 @@ struct PoseOptShared {
   double chi2;
   Solver6 sol;
   double x[8];
-  int done, iters;
+  int done, iters, n_pivoted, cov_pivoted;  // n_pivoted / cov_pivoted: which solves took the fallback (reported)
   unsigned hist[2][256];
   int sel_bin[2], sel_k[2], sel_cnt[2];
 };
@@ -281,7 +281,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
     if (tid == 0) { s.T = T0; s.T_old = T0; s.chi2 = 0.0; }
   }
   if (tid == 0) {
-    s.done = 0; s.iters = 0;
+    s.done = 0; s.iters = 0; s.n_pivoted = 0;
     for (int k = 0; k < 36; ++k) s.A[k] = 0.0;
   }
   po_partials<1>(cnt, s);
@@ -372,6 +372,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
           ldlt6_factor(s.sol.ldl, s.sol.tr);
           for (int k = 0; k < 6; ++k) s.x[k] = b[k];
           ldlt6_solve(s.sol.ldl, s.sol.tr, s.x);
+          s.n_pivoted++;
         }
         __syncwarp();
 #pragma unroll
@@ -449,6 +450,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
     }
     Fact6 F;
     const bool ok = fact6_compute_upper(h, F);
+    if (lane == 0) s.cov_pivoted = ok ? 0 : 1;
     if (ok) {
       double e[6], x[6];
 #pragma unroll
@@ -490,6 +492,8 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
     r.error_final = sqrt(med_final) * fx;
     r.num_obs = (long long)num_obs - (long long)n_deleted;
     r.n_iter_done = s.iters;
+    r.n_pivoted_solves = (int16_t)s.n_pivoted;
+    r.cov_pivoted = (int16_t)s.cov_pivoted;
     P.out[fr] = r;
     pose_to_rt12(s.T, P.T_io + 12 * (size_t)fr);
     PO_DBG(if (fr == 0) printf("[po dbg] N %d iters %d cycles: constants %lld scale-median %lld gauss-newton %lld cull+medians %lld cov+out %lld\n",

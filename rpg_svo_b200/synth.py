@@ -522,6 +522,46 @@ def make_depth_case(seed: int, n_seeds: int = 2000, **kw) -> dict:
     return tv
 
 
+def make_multi_keyframe_depth_case(seed: int, n_seeds: int = 300, n_kfs: int = 3, baseline: float = 0.3) -> dict:
+    """Seeds of n_kfs keyframes with different poses and images (keyframe k moved by up to 15 cm / 3 degrees from
+    keyframe 0), updated by one current frame; ref_index interleaves the keyframes seed by seed (0, 1, 2, 0, 1, ...)."""
+    c = make_depth_case(seed, n_seeds, baseline=baseline)
+    rng = np.random.default_rng(seed + 1000)
+    plane, tex, cam = c["plane"], make_texture(7), c["cam"]
+    kf_T, kf_pyr = [c["T_ref_w"]], [c["ref_pyr"]]
+    for _ in range(1, n_kfs):
+        xi = np.concatenate([rng.uniform(-0.15, 0.15, 3), np.deg2rad(rng.uniform(-3, 3, 3))])
+        T = se3_mul(se3_exp(xi), c["T_ref_w"])
+        kf_T.append(T)
+        kf_pyr.append(build_pyramid(render(cam, T, plane, tex), c["n_levels"]))
+    ref_index = (np.arange(n_seeds) % n_kfs).astype(np.int32)
+    depth_gt = np.array([np.linalg.norm(intersect(plane, kf_T[r], c["ftr_f"][i:i + 1])[0] - se3_inv(kf_T[r])[:, 3])
+                         for i, r in enumerate(ref_index)])
+    c.update(kf_T=kf_T, kf_pyr=kf_pyr, ref_index=ref_index, depth_gt=depth_gt)
+    return c
+
+
+def make_seed_status_case(seed: int, n_seeds: int = 400) -> dict:
+    """One launch's worth of seeds that end in every status DepthFilter::updateSeeds can give them: too old (batch_id),
+    behind the camera (negative mu), outside the current frame (a depth of a few cm, so the current frame's 0.3 m
+    baseline throws the projection off the image or behind it), no match, updated and converged (a fifth of the seeds start
+    at the true depth with a small variance) -- plus seeds whose sigma2 is negative, NaN or infinite."""
+    c = make_depth_case(seed, n_seeds, baseline=0.3)
+    rng = np.random.default_rng(seed + 2000)
+    s = c["seeds"]
+    s["sigma2"][::5] *= np.float32(1e-3)
+    s["mu"][::5] = (1.0 / c["depth_gt"][::5]).astype(np.float32)
+    idx = rng.permutation(n_seeds)
+    s["mu"][idx[:20]] = np.float32(-0.5)                                    # behind
+    s["mu"][idx[20:45]] = rng.uniform(20, 60, 25).astype(np.float32)        # 2-5 cm in front of the keyframe
+    bad = idx[45:75]
+    s["sigma2"][bad] = np.array([-0.1, np.nan, np.inf] * 10, np.float32)
+    c["batch_id"][idx[75:85]] = 0                                           # too old
+    c["bad_sigma2"] = np.zeros(n_seeds, bool)
+    c["bad_sigma2"][bad] = True
+    return c
+
+
 def make_pose_opt_case(seed: int, n: int = 1000, width: int = 1920, height: int = 1080, px_noise: float = 1.0,
                        outlier_frac: float = 0.03) -> dict:
     """BASELINE config C3 (pose optimizer part): n observations with N(0, px_noise) pixel noise
@@ -541,6 +581,42 @@ def make_pose_opt_case(seed: int, n: int = 1000, width: int = 1920, height: int 
     has_point = (rng.uniform(size=n) > 0.02).astype(np.uint8)
     T_init = se3_mul(se3_exp(np.concatenate([rng.uniform(-0.05, 0.05, 3), rng.uniform(-0.01, 0.01, 3)])), T_true)
     return dict(cam=cam, f=f, pos=pos, level=level, has_point=has_point, T_init=T_init, T_true=T_true)
+
+
+def make_pose_window_case(seed: int, n: int, window_px: float, depth: float = 40.0, width: int = 752, height: int = 480,
+                          px_noise: float = 0.3) -> dict:
+    """Ill-conditioned pose problems: n observations inside a window_px x window_px pixel window at the image centre, their
+    points on a fronto-parallel plane `depth` m away.  The smaller the window (and the larger the depth), the closer the
+    translations parallel to the image and the rotations about the two image axes come to explaining the same motion: the
+    normal matrix's smallest unpivoted LDL^T pivot falls with the window."""
+    rng = np.random.default_rng(seed)
+    cam = camera_for(width, height)
+    T_true = base_pose()
+    px = np.stack([rng.uniform(-0.5, 0.5, n), rng.uniform(-0.5, 0.5, n)], axis=1) * window_px + [cam.cx, cam.cy]
+    bearing = cam.cam2world(px)
+    Tinv = se3_inv(T_true)
+    pos = (bearing * (depth / bearing[:, 2:3])) @ Tinv[:, :3].T + Tinv[:, 3]
+    f = cam.cam2world(px + rng.normal(0, px_noise, (n, 2)))
+    level = rng.integers(0, 3, n).astype(np.int32)
+    T_init = se3_mul(se3_exp(np.concatenate([rng.uniform(-0.01, 0.01, 3), rng.uniform(-0.002, 0.002, 3)])), T_true)
+    return dict(cam=cam, f=f, pos=pos, level=level, has_point=np.ones(n, np.uint8), T_init=T_init, T_true=T_true)
+
+
+def make_pose_line_case(seed: int, n: int, width: int = 752, height: int = 480, px_noise: float = 0.3) -> dict:
+    """A singular pose problem: every point on one 3D line through the scene, so the rotation about that line (with the
+    translation that keeps the line in place) does not change any reprojection error."""
+    rng = np.random.default_rng(seed)
+    cam = camera_for(width, height)
+    T_true = base_pose()
+    Tinv = se3_inv(T_true)
+    a, b = np.array([-1.5, -0.4, 3.0]), np.array([1.2, 0.5, 5.0])  # camera-frame end points, in view
+    s = np.sort(rng.uniform(0, 1, n))
+    pos = (a + s[:, None] * (b - a)) @ Tinv[:, :3].T + Tinv[:, 3]
+    px = cam.world2cam(a + s[:, None] * (b - a))
+    f = cam.cam2world(px + rng.normal(0, px_noise, (n, 2)))
+    level = rng.integers(0, 3, n).astype(np.int32)
+    T_init = se3_mul(se3_exp(np.concatenate([rng.uniform(-0.02, 0.02, 3), rng.uniform(-0.004, 0.004, 3)])), T_true)
+    return dict(cam=cam, f=f, pos=pos, level=level, has_point=np.ones(n, np.uint8), T_init=T_init, T_true=T_true)
 
 
 def make_map_case(seed: int, n_kfs: int = 8, n_points: int = 700, width: int = 752, height: int = 480, n_levels: int = 5,

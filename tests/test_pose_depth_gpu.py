@@ -55,6 +55,15 @@ def test_pose_optimize_ties_and_tiny_sets(ctx, oracle):
         assert g["num_obs"] == o["num_obs"] and np.array_equal(g["has_point"], o["has_point"]), n
         for key in ("estimated_scale", "error_init", "error_final"):
             assert abs(g[key] - o[key]) <= 1e-9 * max(1.0, abs(o[key])), (n, key)
+        # with 1-2 observations A is singular (rank 2 / 4): its smallest pivots are rounding noise that the pivoted LDL^T
+        # divides by, in the kernel as in the oracle, so the step -- and the iteration at which chi2 stops falling -- is
+        # decided by each implementation's summation order, and so is whether the Gauss-Jordan inverse meets an exactly
+        # zero pivot (NaN covariance) or a 1e-30 one (huge finite entries); pose and covariance are compared at full rank
+        if n >= 3:
+            assert g["n_iter_done"] == o["n_iter_done"], n
+            dt, dr = synth.pose_error(g["T"], o["T"])
+            assert dt < 1e-8 and dr < 1e-8, (n, dt, dr)
+            assert np.array_equal(np.isfinite(g["cov"]), np.isfinite(o["cov"])), n
 
 
 def test_pose_optimize_no_observations(ctx):
