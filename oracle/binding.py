@@ -692,15 +692,18 @@ def ref_reproject_map(case):
     return trim_reproject(o, st)
 
 
-def fast_detect(pyr, n_pyr_levels, cell_size, detection_threshold, grid_occupancy=None, cap=4096, nonmax_ties_suppress=0):
-    """FastDetector::detect restated: returns dict(x, y, level, score) in grid-cell order."""
+def fast_detect(pyr, n_pyr_levels, cell_size, detection_threshold, grid_occupancy=None, cap=4096, nonmax_ties_suppress=0,
+                fast_threshold=20):
+    """FastDetector::detect restated: returns dict(x, y, level, score) in grid-cell order.  fast_threshold is the FAST
+    segment-test threshold b, which the reference hard-codes to 20."""
     lp, cols, rows = _level_ptrs(pyr)
     h, w = pyr[0].shape
     x, y, lv = np.zeros(cap, np.int32), np.zeros(cap, np.int32), np.zeros(cap, np.int32)
     sc = np.zeros(cap, np.float32)
     occ = None if grid_occupancy is None else np.ascontiguousarray(grid_occupancy, np.uint8)
     n = lib().orc_fast_detect(lp, _p(cols), _p(rows), n_pyr_levels, w, h, cell_size, _p(occ) if occ is not None else None,
-                              C.c_double(detection_threshold), int(nonmax_ties_suppress), _p(x), _p(y), _p(lv), _p(sc), cap)
+                              C.c_double(detection_threshold), int(fast_threshold), int(nonmax_ties_suppress), _p(x), _p(y),
+                              _p(lv), _p(sc), cap)
     assert n <= cap
     return dict(x=x[:n], y=y[:n], level=lv[:n], score=sc[:n])
 

@@ -247,14 +247,14 @@ void orc_reproject_map(const orc_map_view* map, const uint8_t* const* kf_levels 
                        double* new_px, int* new_level, int* new_type, double* new_grad, orc_reproject_stats* stats);
 
 /* ---- feature_detection::FastDetector::detect (svo/src/feature_detection.cpp:66-115) ----
- * FAST-10 (b = 20) + score + 3x3 non-maximum suppression per pyramid level, Shi-Tomasi score per surviving corner, best
- * corner per grid cell over all levels, cells flagged in grid_occupancy (NULL = none) skipped.  The `fast` library and
- * vk::shiTomasiScore are [EXT] (oracle/fast_ext.h).  Output: corners in cell order (level-0 pixel coordinates, level,
- * score); returns their number (may exceed cap; only cap are written). */
+ * FAST-10 (b = fast_threshold; the reference hard-codes 20) + score + 3x3 non-maximum suppression per pyramid level,
+ * Shi-Tomasi score per surviving corner, best corner per grid cell over all levels, cells flagged in grid_occupancy
+ * (NULL = none) skipped.  The `fast` library and vk::shiTomasiScore are [EXT] (oracle/fast_ext.h).  Output: corners in
+ * cell order (level-0 pixel coordinates, level, score); returns their number (may exceed cap; only cap are written). */
 int orc_fast_detect(const uint8_t* const* levels, const int* cols, const int* rows, int n_pyr_levels, int img_width,
                     int img_height, int cell_size, const uint8_t* grid_occupancy, double detection_threshold,
-                    int nonmax_ties_suppress /*[EXT] 0 = libCVD non-strict (default)*/, int* out_x, int* out_y,
-                    int* out_level, float* out_score, int cap);
+                    int fast_threshold, int nonmax_ties_suppress /*[EXT] 0 = libCVD non-strict (default)*/, int* out_x,
+                    int* out_y, int* out_level, float* out_score, int cap);
 
 #ifdef __cplusplus
 }

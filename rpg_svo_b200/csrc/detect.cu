@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) fast_detect_kernel(DetectLevels lv, int b
   for (int i = threadIdx.x; i < kScH * kScW; i += blockDim.x) {
     const int sy = i / kScW, sx = i - sy * kScW;
     const int gx = x0 - 1 + sx, gy = y0 - 1 + sy;
-    int score = 0;
+    int score = -1;  // not a corner; corner scores lie in [b, 254], and b may be 0
     if (gx >= 3 && gx < W - 3 && gy >= 3 && gy < H - 3) {  // fast_corner_detect_10: 3-pixel border
       const int lx = sx + kHalo - 1, ly = sy + kHalo - 1;
       const int c = img[ly][lx];
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(256) fast_detect_kernel(DetectLevels lv, int b
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int gx = x0 + tx, gy = y0 + ty;
   const int s = sc[ty + 1][tx + 1];
-  if (s == 0 || gx >= W || gy >= H) return;
+  if (s < 0 || gx >= W || gy >= H) return;
   // fast_nonmax_3x3: suppressed by a detected neighbour whose score compares >= (ties suppress) or >
   bool bad = false;
 #pragma unroll
@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(256) fast_detect_kernel(DetectLevels lv, int b
     for (int dx = -1; dx <= 1; ++dx) {
       if (dx == 0 && dy == 0) continue;
       const int n = sc[ty + 1 + dy][tx + 1 + dx];
-      if (n != 0 && (ties_suppress ? n >= s : n > s)) bad = true;
+      if (n >= 0 && (ties_suppress ? n >= s : n > s)) bad = true;
     }
   if (bad) return;
   const int scale = 1 << L;
@@ -179,7 +179,9 @@ extern "C" int svo_b200_fast_detect(svo_b200_ctx* ctx, const svo_b200_frame* fra
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
   uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  const float thr_f = (float)opt->detection_threshold;  // Corner(0,0,detection_threshold,0,0.0f): stored as float (:72)
+  float thr_f = (float)opt->detection_threshold;  // Corner(0,0,detection_threshold,0,0.0f): stored as float (:72)
+  // -0.0 compares like +0.0, but its sign bit would make the initial key larger than every positive score's key
+  if (thr_f == 0.0f) thr_f = 0.0f;
   unsigned thr_bits;
   std::memcpy(&thr_bits, &thr_f, 4);
   const unsigned long long init = ((unsigned long long)thr_bits << 32) | 0xffffffffull;
@@ -195,11 +197,12 @@ extern "C" int svo_b200_fast_detect(svo_b200_ctx* ctx, const svo_b200_frame* fra
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_cells, d + o_cells, sizeof(unsigned long long) * n_cells, cudaMemcpyDeviceToHost, ctx->stream));
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  // corners with a high enough score, in cell order (:106-110)
+  // corners with a high enough score, in cell order (:106-110).  A cell no corner beat still holds the initial
+  // Corner(0, 0, detection_threshold, 0): it decodes to (0, 0), level 0, and passes the check whenever the float32
+  // threshold rounded above the double one -- the reference then emits it too.
   int n = 0;
   for (int k = 0; k < n_cells; ++k) {
     const unsigned long long key = reinterpret_cast<const unsigned long long*>(h + o_cells)[k];
-    if (key == init) continue;
     const unsigned bits = (unsigned)(key >> 32);
     float score;
     std::memcpy(&score, &bits, 4);

@@ -47,15 +47,9 @@ struct ReprojOut {
 };
 
 __global__ void __launch_bounds__(kRpWarps * 32) reproject_match_kernel(
-    FrameDesc cur, Cam cam, int E, int n_kfs, ReprojIn in, ReprojOut out, const double* __restrict__ cur_T_f_w, int cell_size,
+    FrameDesc cur, Cam cam, int E, ReprojIn in, ReprojOut out, const double* __restrict__ cur_T_f_w, int cell_size,
     int grid_n_cols, int find_match, int max_search_level, int align_max_iter) {
-  extern __shared__ double kf_pos[];  // n_kfs*3: Frame::pos() = T_f_w_.inverse().translation()
   __shared__ WarpAlignScratch scratch[kRpWarps];
-  for (int k = threadIdx.x; k < n_kfs; k += blockDim.x) {
-    const Pose Ti = pose_inv(pose_from_rt12(in.kf_T + 12 * (size_t)k));
-    kf_pos[3 * k] = Ti.t[0]; kf_pos[3 * k + 1] = Ti.t[1]; kf_pos[3 * k + 2] = Ti.t[2];
-  }
-  __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int e = blockIdx.x * kRpWarps + warp;
   if (e >= E) return;
@@ -81,8 +75,11 @@ __global__ void __launch_bounds__(kRpWarps * 32) reproject_match_kernel(
     double best_c = 0.0;
     int best_j = b;
     for (int j = b + lane; j < en; j += 32) {
+      // Frame::pos() = T_f_w_.inverse().translation() of the observing keyframe, computed by the lane that reads it:
+      // nothing is staged per keyframe, so the number of keyframes in the map view has no limit
       const int k = in.ftr_kf[in.pt_obs[j]];
-      double dx = kf_pos[3 * k] - pos[0], dy = kf_pos[3 * k + 1] - pos[1], dz = kf_pos[3 * k + 2] - pos[2];
+      const Pose Ti = pose_inv(pose_from_rt12(in.kf_T + 12 * (size_t)k));
+      double dx = Ti.t[0] - pos[0], dy = Ti.t[1] - pos[1], dz = Ti.t[2] - pos[2];
       const double dn = sqrt(dx * dx + dy * dy + dz * dz);
       dx /= dn; dy /= dn; dz /= dn;
       const double c = ox * dx + oy * dy + oz * dz;
@@ -267,8 +264,8 @@ extern "C" int svo_b200_reproject_map(svo_b200_ctx* ctx, const svo_b200_map_view
                    reinterpret_cast<int*>(d + o_rf)};
   const int blocks = (E + kRpWarps - 1) / kRpWarps;
   kt_begin(ctx);
-  reproject_match_kernel<<<blocks, kRpWarps * 32, sizeof(double) * 3 * m->n_kfs, ctx->stream>>>(
-      make_desc(cur), cm, E, m->n_kfs, in, out, reinterpret_cast<const double*>(d + o_cT), cell_size, grid_n_cols,
+  reproject_match_kernel<<<blocks, kRpWarps * 32, 0, ctx->stream>>>(
+      make_desc(cur), cm, E, in, out, reinterpret_cast<const double*>(d + o_cT), cell_size, grid_n_cols,
       opt->find_match_direct, opt->max_search_level, opt->align_max_iter);
   ctx->launches++;
   kt_end(ctx);

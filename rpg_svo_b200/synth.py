@@ -620,12 +620,15 @@ def make_pose_line_case(seed: int, n: int, width: int = 752, height: int = 480, 
 
 
 def make_map_case(seed: int, n_kfs: int = 8, n_points: int = 700, width: int = 752, height: int = 480, n_levels: int = 5,
-                  n_candidates: int = 80, spread: float = 0.5, bad_frac: float = 0.2, cam: Camera | None = None) -> dict:
+                  n_candidates: int = 80, spread: float = 0.5, bad_frac: float = 0.2, cam: Camera | None = None,
+                  obs_prob: float = 0.45, same_pose: tuple = ()) -> dict:
     """A small map for Reprojector::reprojectMap (svo/src/reprojector.cpp:64-217): n_kfs keyframes on a trajectory above
     the textured plane, world points on the plane observed by 1..n_kfs keyframes (one Feature per observation, detected
     on the integer grid of its level), point types / reprojection counters near the reference's thresholds, converged-
     seed candidates whose single observation is not in its keyframe's fts_ list, five key points per keyframe, a current
-    frame close to the last keyframes, and a shuffled cell order.  Everything is flat arrays (the `map view`)."""
+    frame close to the last keyframes, and a shuffled cell order.  Everything is flat arrays (the `map view`).
+    obs_prob: the probability that a keyframe observes a map point.  same_pose: (src, dst) keyframe pairs; keyframe dst
+    gets the pose (and image) of keyframe src, so Point::getCloseViewObs sees exactly equal angles."""
     rng = np.random.default_rng(seed)
     cam = camera_for(width, height) if cam is None else cam
     plane, tex = Plane.tilted(), make_texture(7)
@@ -633,6 +636,8 @@ def make_map_case(seed: int, n_kfs: int = 8, n_points: int = 700, width: int = 7
     for k in range(n_kfs):
         xi = np.concatenate([rng.uniform(-spread, spread, 2), rng.uniform(-0.15, 0.15, 1), np.deg2rad(rng.uniform(-3, 3, 3))])
         kf_T.append(se3_mul(se3_exp(xi), base_pose()))
+    for src, dst in same_pose:
+        kf_T[dst] = kf_T[src].copy()
     xi = np.concatenate([rng.uniform(-0.1, 0.1, 3), np.deg2rad(rng.uniform(-2, 2, 3))])
     cur_T = se3_mul(se3_exp(xi), kf_T[-1])
     kf_pyr = [build_pyramid(render(cam, T, plane, tex), n_levels) for T in kf_T]
@@ -673,7 +678,7 @@ def make_map_case(seed: int, n_kfs: int = 8, n_points: int = 700, width: int = 7
 
     for p in range(n_points):
         for k in range(n_kfs):
-            if rng.uniform() < 0.45:
+            if rng.uniform() < obs_prob:
                 add_ftr(k, p, True)
     cand = []
     for p in range(n_points, P):

@@ -65,3 +65,58 @@ def test_depth_seed_statuses_oracle_equals_reference(oracle, ref):
     keep = r["status"] == 0
     for k in ("a", "b", "mu", "z_range", "sigma2"):
         assert np.array_equal(r[k][keep].view(np.uint32), o[k][keep].view(np.uint32)), k
+
+
+@pytest.mark.parametrize("kind", ["render", "noise", "checker", "low_contrast"])
+def test_fast_numpy_statement_equals_oracle(oracle, kind):
+    """The oracle's detector against the independent numpy statement (tests/fast_numpy.py: the segment test from the
+    ring's definition, the library's literal bisection, dense 3x3 suppression, Shi-Tomasi in float64) for every FAST
+    threshold b from 0 to 254 and both tie modes.  x, y and level must agree on every cell float64 decides."""
+    from tests import fast_numpy as fn
+
+    pyr = fn.images(1)[kind]
+    n_corners = 0
+    for b in (0, 1, 19, 20, 21, 60, 200, 254):
+        for ties in (0, 1):
+            r = fn.detect(pyr, 3, 8, 0.0, b=b, ties_suppress=bool(ties))
+            o = oracle.fast_detect(pyr, 3, 8, 0.0, nonmax_ties_suppress=ties, fast_threshold=b)
+            assert len(r["ambiguous"]) <= 2
+            assert fn.agree(r, o, 64, 8) >= 46
+            n_corners += len(o["x"])
+            if kind == "low_contrast" and b == 0:
+                assert (r["fast_score"] == 0).sum() >= 20                    # score-0 corners win their cells
+    assert n_corners > 0
+
+
+def test_fast_detect_thresholds_oracle_equals_reference(oracle, ref):
+    """The compiled reference's FastDetector (b = 20, as it hard-codes) on a tiled 16x16 motif, whose cells hold equal
+    Shi-Tomasi scores, and at detection thresholds around a winner's float32 score.  A threshold whose float32 rounding
+    lies above it leaves the initial Corner(0, 0, threshold, 0) of every cell no corner beat above the threshold, and the
+    reference emits it."""
+    motif = np.random.default_rng(4).integers(0, 256, (16, 16), dtype=np.uint8)
+    pyr = synth.build_pyramid(np.tile(motif, (6, 8)), 3)
+    a, b = oracle.fast_detect(pyr, 3, 32, 0.0), ref.fast_detect(pyr[0], 3, 3, 32, 0.0)
+    assert all(np.array_equal(a[k], b[k]) for k in ("x", "y", "level")) and len(a["x"]) == 12
+    pyr = synth.make_two_view(5, width=320, height=240, n_levels=3)["ref_pyr"]
+    s = float(np.median(oracle.fast_detect(pyr, 3, 30, 0.0)["score"]))
+    for thr in (0.0, -0.0, s, np.nextafter(s, np.inf), np.nextafter(s, -np.inf), 1e30):
+        a, b = oracle.fast_detect(pyr, 3, 30, thr), ref.fast_detect(pyr[0], 3, 3, 30, float(thr))
+        assert all(np.array_equal(a[k], b[k]) for k in ("x", "y", "level")), thr
+    assert ((b["x"] == 0) & (b["y"] == 0)).sum() == 11 * 8                    # 1e30: placeholders only
+
+
+def test_many_observations_reprojection_oracle_equals_reference(oracle, ref):
+    """Points with 32 to ~70 observations, exactly equal viewing angles (duplicated keyframe poses) and points seen
+    only from behind: Point::getCloseViewObs and the cell policy of the compiled reference against the oracle."""
+    from tests import reproject_cases as rc
+
+    c = rc.many_obs_case()
+    c = dict(c, options=dict(c["options"], max_fts=1000))
+    r, o = ref.reproject_map(c), oracle.reproject_map(c)
+    for k in ("n_matches", "n_trials", "n_new", "n_overlap"):
+        assert r[k] == o[k], k
+    for k in ("overlap_kf", "overlap_count", "new_point", "new_level", "new_type", "pt_type", "pt_n_failed", "pt_n_succeeded"):
+        assert np.array_equal(r[k], o[k]), k
+    assert np.max(np.abs(r["new_px"] - o["new_px"]), initial=0.0) <= 1e-9
+    assert np.allclose(r["new_grad"], o["new_grad"], rtol=0, atol=1e-9)
+    assert o["n_new"] > 30
