@@ -207,6 +207,16 @@ __device__ __forceinline__ void fetch12(const uint8_t* base, int off, uint32_t& 
   hi = __funnelshift_r(w1, w2, sh);
 }
 
+// Element k of a per-feature register array, read with compile-time indices only: in a loop over the thread's features that
+// is not unrolled, a[k] would put the whole array in local memory.
+template <class T, int FPT>
+__device__ __forceinline__ T sel_k(const T (&a)[FPT], int k) {
+  T v = a[0];
+#pragma unroll
+  for (int j = 1; j < FPT; ++j) v = k == j ? a[j] : v;
+  return v;
+}
+
 // per-feature unscaled Jacobian rows: a = row0 of jacobian_xyz2uv, b = row1 (frame.h:116-138)
 __device__ __forceinline__ void jac_rows(double x, double y, double zi, double (&a)[6], double (&b)[6]) {
   const double X = x * zi, Y = y * zi;
@@ -830,21 +840,41 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       }
     }
   };
+  // ---- gradient moments Sxx, Sxy, Syy of this thread's patches in `mask` (zero for the others), summed pixel by pixel from
+  //      the gradient array pd in shared memory
+  auto patch_moments = [&](const float2* pd, const unsigned mask, double (&sxx)[FPT], double (&sxy)[FPT], double (&syy)[FPT]) {
+#pragma unroll
+    for (int k = 0; k < FPT; ++k) {
+      sxx[k] = sxy[k] = syy[k] = 0.0;
+      if (!((mask >> k) & 1u)) continue;
+      const int slot = tid + k * T;
+#pragma unroll
+      for (int p = 0; p < kPatchArea; ++p) {
+        const float2 gr = pd[p * SA + slot];
+        const double dx = (double)gr.x, dy = (double)gr.y;
+        sxx[k] = fma(dx, dx, sxx[k]);
+        sxy[k] = fma(dx, dy, sxy[k]);
+        syy[k] = fma(dy, dy, syy[k]);
+      }
+    }
+  };
   // ---- precomputeReferencePatches (:84-145) of one level into the patch arrays (pr, pd): visibility bits, the f32 patch and
   //      its gradients, and the per-feature gradient moments m_* the H reduction needs.  `with_windows`: also request the
   //      current-image windows (between the footprint loads and the arithmetic, so that both latencies overlap).
+  //      Throughput geometry: the loop over the thread's features is not unrolled, so moments stored here would be indexed by
+  //      the feature and live in local memory, which misses the small L1 left beside 3 x 75 KB of shared memory; it leaves
+  //      m_* alone and the caller sums them afterwards with patch_moments(pd, vis_mask) -- a visible patch has its gradients
+  //      in pd (zero for a stale one), summed in the same order.  The other geometries unroll the loop and keep the moments of
+  //      the patch arithmetic (a second pass over pd would lengthen the latency path of the cluster geometries).
   auto level_patches = [&](const int level, float* pr, float2* pd, const float* pr_stale, const int mode, const bool with_windows,
-                           double (&m_sxx)[FPT], double (&m_sxy)[FPT], double (&m_syy)[FPT], double (&m_cnt)[FPT]) {
+                           double (&m_sxx)[FPT], double (&m_sxy)[FPT], double (&m_syy)[FPT]) {
     const int W = P.w[level], Hh = P.h[level];
     const float scale = 1.0f / (float)(1 << level);
     const uint8_t* ref_img = job.ref_lvl[level];
     const uint8_t* cur_img = job.cur_lvl[level];
-    // (throughput geometry: a loop over the thread's features -- the per-feature moments m_* are then indexed dynamically and
-    // live in local memory, eight values per level, which is cheaper than a second copy of the patch arithmetic in the
-    // instruction stream)
 #pragma unroll(SS ? 1 : FPT)
     for (int k = 0; k < FPT; ++k) {
-      m_sxx[k] = m_sxy[k] = m_syy[k] = m_cnt[k] = 0.0;
+      if constexpr (!SS) m_sxx[k] = m_sxy[k] = m_syy[k] = 0.0;
       const int slot = tid + k * T;
       // px is re-read from the pair's blob in global memory (L2) once per level instead of living in registers
       const double2 pxy = slot < n_loc ? __ldg(reinterpret_cast<const double2*>(job.blob) + fbase + slot) : make_double2(-1e6, -1e6);
@@ -908,7 +938,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
 #pragma unroll
           for (int c = 0; c < 7; ++c) pr0[c] = pr1[c];
         }
-        m_sxx[k] = sxx; m_sxy[k] = sxy; m_syy[k] = syy; m_cnt[k] = 1.0;
+        if constexpr (!SS) { m_sxx[k] = sxx; m_sxy[k] = sxy; m_syy[k] = syy; }
       } else if ((vis_mask >> k) & 1u) {
         // visible from a coarser level but failing here: the reference would keep the stale patch
         // and a zeroed Jacobian (jacobian_cache_.setZero() per level, :64).  Unreachable for
@@ -917,7 +947,6 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         for (int p = 0; p < kPatchArea; ++p) pd[p * SA + slot] = make_float2(0.f, 0.f);
         if (pr_stale)  // per-level arrays (upfront variant): the stale patch is the previous level's
           for (int p = 0; p < kPatchArea; ++p) pr[p * SA + slot] = pr_stale[p * SA + slot];
-        m_cnt[k] = 1.0;
       }
     }
   };
@@ -932,13 +961,13 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     // ---- all levels' reference patches and per-warp H partials, coarse to fine (the visibility mask accumulates in that order)
     for (int level = lvl_hi; level >= lvl_lo; --level) {
       const int li = lvl_hi - level;
-      double m_sxx[FPT], m_sxy[FPT], m_syy[FPT], m_cnt[FPT];
+      double m_sxx[FPT], m_sxy[FPT], m_syy[FPT];
       level_patches(level, pat_ref_of(li), pat_dxy_of(li), li > 0 ? pat_ref_of(li - 1) : (const float*)nullptr, kModeGlobal, false,
-                    m_sxx, m_sxy, m_syy, m_cnt);
+                    m_sxx, m_sxy, m_syy);
       vis_levels |= (vis_mask & 1u) << li;
       warp_h_partials<FPT, false>(
           [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
-            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = m_sxx[k]; sxy = m_sxy[k]; syy = m_syy[k]; cnt = m_cnt[k];
+            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = sel_k(m_sxx, k); sxy = sel_k(m_sxy, k); syy = sel_k(m_syy, k); cnt = ((vis_mask >> k) & 1u) ? 1.0 : 0.0;
           },
           &up.hpart[li][warp * kPartK]);
     }
@@ -1003,12 +1032,13 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     if constexpr (!UP) {
       // ---- precomputeReferencePatches (:84-145), one feature per thread; the windows of the current image are requested
       //      between the footprint loads and the patch arithmetic
-      double m_sxx[FPT], m_sxy[FPT], m_syy[FPT], m_cnt[FPT];
-      level_patches(level, pat_ref, pat_dxy, (const float*)nullptr, mode, true, m_sxx, m_sxy, m_syy, m_cnt);
+      double m_sxx[FPT], m_sxy[FPT], m_syy[FPT];
+      level_patches(level, pat_ref, pat_dxy, (const float*)nullptr, mode, true, m_sxx, m_sxy, m_syy);
+      if constexpr (SS) patch_moments(pat_dxy, vis_mask, m_sxx, m_sxy, m_syy);
       SIA_DBG(if ((SVO_SIA_DEBUG && P.debug) && tid == 0) { tq1 = clock64(); s.tk[7] += tq1 - tq0; })
       pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
           [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
-            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = m_sxx[k]; sxy = m_sxy[k]; syy = m_syy[k]; cnt = m_cnt[k];
+            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = sel_k(m_sxx, k); sxy = sel_k(m_sxy, k); syy = sel_k(m_syy, k); cnt = ((vis_mask >> k) & 1u) ? 1.0 : 0.0;
             // opaque to the optimiser: otherwise the level-invariant Jacobian rows are hoisted out of the level loop and
             // parked in local memory (17 doubles per thread, written once and re-read every level)
             asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));
@@ -1196,23 +1226,10 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       // contributed in this pass ("slow path"; all threads, one block barrier inside)
       auto slow_sum_h = [&]() {
         double q_sxx[FPT], q_sxy[FPT], q_syy[FPT];
-#pragma unroll
-        for (int k = 0; k < FPT; ++k) {
-          q_sxx[k] = q_sxy[k] = q_syy[k] = 0.0;
-          if (!((in_mask >> k) & 1u)) continue;
-          const int slot = tid + k * T;
-#pragma unroll
-          for (int p = 0; p < kPatchArea; ++p) {
-            const float2 gr = pat_dxy[p * SA + slot];
-            const double dx = (double)gr.x, dy = (double)gr.y;
-            q_sxx[k] = fma(dx, dx, q_sxx[k]);
-            q_sxy[k] = fma(dx, dy, q_sxy[k]);
-            q_syy[k] = fma(dy, dy, q_syy[k]);
-          }
-        }
+        patch_moments(pat_dxy, in_mask, q_sxx, q_sxy, q_syy);
         pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
             [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
-              { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = q_sxx[k]; sxy = q_sxy[k]; syy = q_syy[k]; cnt = 0.0;
+              { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = sel_k(q_sxx, k); sxy = sel_k(q_sxy, k); syy = sel_k(q_syy, k); cnt = 0.0;
               asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));  // see the per-level call: no hoisting into local memory
             },
             s, nwarps, P.xg, pair);
