@@ -100,7 +100,6 @@ struct SiaParams {
   int max_level, min_level, n_iter;
   double eps;
   int stage_cap;  // bytes of the staging region in shared memory (TMA image / cp.async windows)
-  int slots;      // blockDim * FPT feature slots per CTA (patch arrays are [3][16][slots])
   double* T_out;
   double* H_out;
   uint8_t* visible_out;
@@ -592,6 +591,41 @@ __device__ __forceinline__ void sia_world2cam(const CamDev& c, double x, double 
   }
 }
 
+// Feature slots of the throughput geometry's shared arrays (the host selects it for at most this many features per pair).
+constexpr int kSiaThroughputSlots = 304;
+
+// One instantiation of sia_kernel (EVAL aside): its template arguments and the shared-memory layout that follows from them.
+// The kernel finds its regions with it and the host (kSiaEntries) sizes and reports launches with it.
+template <int FPT_, int MAXT_, int MINB_, int CS_, bool CG_, bool UP_>
+struct SiaInst {
+  static constexpr int FPT = FPT_, MAXT = MAXT_, MINB = MINB_, CS = CS_;
+  static constexpr bool CG = CG_, UP = UP_;
+  static constexpr int NWC = MAXT / 32;  // warps of one CTA; the host launches exactly MAXT threads
+  // Throughput geometry (160 threads x 2 features, three CTAs per SM): the shared arrays are allocated for
+  // kSiaThroughputSlots slots, which leaves room for the per-feature state xyz_ref in shared memory next to the two coarsest
+  // current images.  Kept in registers that state was spilled at 128 registers per thread, and local memory misses the small
+  // L1 left beside 3 x 75 KB of shared memory (each miss at the head of a feature's projection chain).
+  static constexpr bool SS = FPT == 2 && MAXT == 160 && CS == 1;
+  static constexpr int SA = SS ? kSiaThroughputSlots : MAXT * FPT;  // stride of the per-slot shared arrays
+  // The throughput geometry has no room for windows (its staging region holds the two coarsest current images) and is never
+  // used for the multi-GPU feature split: both code paths are compiled out of it, and its residual pass loops over the
+  // thread's features instead of being unrolled -- the instruction stream of one Gauss-Newton iteration shrinks from ~27 KB to
+  // ~20 KB, which matters with three CTAs in different phases sharing one instruction cache.
+  static constexpr bool WIN = !SS;  // per-feature cp.async windows of the current image exist in this instantiation
+  static constexpr bool XG = CS == 1 && !SS;  // multi-GPU feature split (svo_b200_sia_split_*) compiled in
+  using SH = SiaSharedT<NWC, CS>;
+  using UPT = SiaUpT<NWC, CS>;
+  // dynamic shared memory: control block (SH, then UPT when UP), patch array sets, xyz_ref (SS), staging region
+  static constexpr size_t kShBytes = (sizeof(SH) + 15) & ~size_t(15);
+  static constexpr size_t kCtlBytes = kShBytes + (UP ? ((sizeof(UPT) + 15) & ~size_t(15)) : 0);
+  static constexpr size_t kSetFloats = (size_t)3 * kPatchArea * SA;  // one set: [16][SA] f32 patch, [16][SA] float2 gradients
+  static constexpr size_t kXyzDoubles = SS ? (size_t)3 * SA : 0;     // [3][SA] f64 xyz_ref
+  // bytes in front of the staging region with n_sets patch array sets (1, or one per level when UP)
+  static constexpr size_t fixed_bytes(int n_sets) {
+    return kCtlBytes + (size_t)n_sets * kSetFloats * sizeof(float) + kXyzDoubles * sizeof(double);
+  }
+};
+
 // One CTA (CS == 1) or one cluster of CS CTAs per frame pair; the pair's features are dealt to the CTAs in
 // contiguous blocks of S = MAXT*FPT slots.
 // (__launch_bounds__(160, 3) yields 128 registers although 3 x 160 x 136 <= 64 K: the register file is split over the
@@ -605,47 +639,32 @@ __device__ __forceinline__ void sia_world2cam(const CamDev& c, double x, double 
 //
 // UP = true (cluster geometry, every CTA alone on its SM): patches / H / factorisations of all levels are computed before
 // the first iteration (SiaUpT); shared memory then holds one patch array set per level.
-// Compile-time layout of one instantiation (explained where the kernel uses it); the host reports launches with it.
-template <int FPT, int MAXT, int CS>
-struct SiaLayout {
-  static constexpr bool SS = (FPT == 2 && MAXT == 160 && CS == 1);
-  static constexpr int SA = SS ? 304 : MAXT * FPT;
-  static constexpr bool WIN = !SS;
-};
-
 template <int FPT, bool EVAL, int MAXT, int MINB, int CS, bool CG, bool UP>
 __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   static_assert(!UP || (CS > 1 && FPT == 1 && !EVAL), "the upfront variant exists for the cluster geometry only");
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  using SH = SiaSharedT<MAXT / 32, CS>;
-  using UPT = SiaUpT<MAXT / 32, CS>;
-  using LAY = SiaLayout<FPT, MAXT, CS>;
+  using G = SiaInst<FPT, MAXT, MINB, CS, CG, UP>;
+  using SH = typename G::SH;
+  using UPT = typename G::UPT;
   SH& s = *reinterpret_cast<SH*>(smem_raw);
-  constexpr int S = MAXT * FPT;  // feature slots of this CTA (== P.slots, checked on the host)
-  // Throughput geometry (160 threads x 2 features, three CTAs per SM): the shared arrays are allocated for SA = 304 slots
-  // (the host selects it for <= 304 features only), which leaves room for the per-feature state xyz_ref in shared memory
-  // next to the two coarsest current images.  Kept in registers that state was spilled at 128 registers per thread, and local
-  // memory misses the small L1 left beside 3 x 75 KB of shared memory (each miss at the head of a feature's projection chain).
-  constexpr bool SS = LAY::SS;
-  constexpr int SA = LAY::SA;  // stride of the per-slot shared arrays
-  // The throughput geometry has no room for windows (its staging region holds the two coarsest current images) and is never
-  // used for the multi-GPU feature split: both code paths are compiled out of it, and its residual pass loops over the
-  // thread's features instead of being unrolled -- the instruction stream of one Gauss-Newton iteration shrinks from ~27 KB to
-  // ~20 KB, which matters with three CTAs in different phases sharing one instruction cache.
-  constexpr bool WIN = LAY::WIN;  // per-feature cp.async windows of the current image exist in this instantiation
-  constexpr bool XG = (CS == 1) && !SS;  // multi-GPU feature split (svo_b200_sia_split_*) compiled in
-  constexpr size_t kCtlBytes = ((sizeof(SH) + 15) & ~size_t(15)) + (UP ? ((sizeof(UPT) + 15) & ~size_t(15)) : 0);
-  UPT& up = *reinterpret_cast<UPT*>(smem_raw + ((sizeof(SH) + 15) & ~size_t(15)));  // only touched when UP
+  constexpr int S = MAXT * FPT;  // feature slots of this CTA
+  constexpr bool SS = G::SS;
+  constexpr int SA = G::SA;
+  constexpr bool WIN = G::WIN;
+  constexpr bool XG = G::XG;
+  UPT& up = *reinterpret_cast<UPT*>(smem_raw + G::kShBytes);  // only touched when UP
   const int n_lvl_bufs = UP ? (P.max_level - P.min_level + 1) : 1;  // patch array sets (one per level when UP)
-  float* const pat_base = reinterpret_cast<float*>(smem_raw + kCtlBytes);
-  // set li (0 = coarsest level) : [16][S] f32 reference patch, then [16][S] float2 gradients
-  auto pat_ref_of = [&](int li) -> float* { return pat_base + (size_t)li * 3 * kPatchArea * SA; };
+  // the regions in the order of SiaInst::fixed_bytes (pointer steps in the regions' element types: stepping in bytes
+  // instead changes the generated address arithmetic)
+  float* const pat_base = reinterpret_cast<float*>(smem_raw + G::kCtlBytes);
+  // set li (0 = coarsest level) : [16][SA] f32 reference patch, then [16][SA] float2 gradients
+  auto pat_ref_of = [&](int li) -> float* { return pat_base + (size_t)li * G::kSetFloats; };
   auto pat_dxy_of = [&](int li) -> float2* { return reinterpret_cast<float2*>(pat_ref_of(li) + kPatchArea * SA); };
   float* pat_ref = pat_ref_of(0);
   float2* pat_dxy = pat_dxy_of(0);
-  double* const st_xyz = reinterpret_cast<double*>(pat_base + (size_t)n_lvl_bufs * 3 * kPatchArea * SA);  // SS: [3][SA] xyz_ref
-  uint8_t* stage = reinterpret_cast<uint8_t*>(st_xyz + (SS ? 3 * SA : 0));  // 16-byte aligned
-  uint4* win = reinterpret_cast<uint4*>(stage);                                                      // [kWinRows][S] 16-byte window rows
+  double* const st_xyz = reinterpret_cast<double*>(pat_base + (size_t)n_lvl_bufs * G::kSetFloats);  // SS: [3][SA] xyz_ref
+  uint8_t* stage = reinterpret_cast<uint8_t*>(st_xyz + G::kXyzDoubles);  // 16-byte aligned
+  uint4* win = reinterpret_cast<uint4*>(stage);                                                      // [kWinRows][SA] 16-byte window rows
 
   const unsigned crank = CS == 1 ? 0u : cluster_rank();
   const int pair = CS == 1 ? (int)blockIdx.x : (int)(blockIdx.x / CS);
@@ -1384,6 +1403,49 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
 // =============================================================================================
 // Host side
 // =============================================================================================
+using SiaKernel = void (*)(SiaParams);
+
+// What the host needs of one alignment instantiation (SiaInst), and its kernels.
+struct SiaEntry {
+  int fpt, threads, min_blocks, cluster;              // FPT, MAXT (the block size), MINB (resident CTAs per SM), CS
+  bool general_camera, upfront, throughput, windows;  // CG, UP, SS, WIN
+  int slots;                                          // SA
+  size_t (*fixed_bytes)(int n_sets);
+  SiaKernel kern[2];  // EVAL = false / true (no residual pass: nullptr)
+};
+
+template <int FPT, int MAXT, int MINB, int CS, bool CG, bool UP>
+static SiaEntry sia_entry() {
+  using G = SiaInst<FPT, MAXT, MINB, CS, CG, UP>;
+  SiaKernel eval = nullptr;
+  if constexpr (CG && !UP) eval = sia_kernel<FPT, true, MAXT, MINB, CS, CG, UP>;
+  return {FPT, MAXT, MINB, CS, CG, UP, G::SS, G::WIN, G::SA, G::fixed_bytes, {sia_kernel<FPT, false, MAXT, MINB, CS, CG, UP>, eval}};
+}
+
+// Every alignment instantiation.  pick_launch takes the first general-camera, per-level entry that fits, so the one-CTA
+// entries are in the order it tries them.  The undistorted pinhole has its own instantiation of the geometries that carry the
+// throughput / latency figures; the residual pass and the rarely used geometries run the general-camera code only.
+static const SiaEntry kSiaEntries[] = {
+    sia_entry<1, 96, 2, 2, true, false>(),
+    sia_entry<1, 96, 2, 4, true, false>(),  sia_entry<1, 96, 2, 4, false, false>(),
+    sia_entry<1, 96, 1, 4, true, true>(),   sia_entry<1, 96, 1, 4, false, true>(),
+    sia_entry<1, 96, 2, 8, true, false>(),
+    sia_entry<2, 160, 3, 1, true, false>(), sia_entry<2, 160, 3, 1, false, false>(),
+    sia_entry<1, 320, 2, 1, true, false>(), sia_entry<1, 320, 2, 1, false, false>(),
+    sia_entry<1, 384, 2, 1, true, false>(),
+    sia_entry<1, 512, 1, 1, true, false>(),
+    sia_entry<2, 512, 1, 1, true, false>(),
+};
+
+// The entry of e's geometry (CTAs per pair, threads, features per thread) with the given camera and upfront flags.
+static const SiaEntry* sia_variant(const SiaEntry& e, bool general_camera, bool upfront) {
+  for (const SiaEntry& v : kSiaEntries)
+    if (v.cluster == e.cluster && v.threads == e.threads && v.fpt == e.fpt && v.general_camera == general_camera &&
+        v.upfront == upfront)
+      return &v;
+  return nullptr;
+}
+
 struct SiaBatchState {
   int B = 0;
   int total_feat = 0;
@@ -1396,8 +1458,7 @@ struct SiaBatchState {
   DevBuf d_in, d_out;
   HostBuf h_in, h_out;
   size_t o_T = 0, o_H = 0, o_vis = 0, o_stats = 0, out_bytes = 0;
-  int threads = 0, fpt = 1, cluster = 1;
-  bool upfront = false;  // cluster geometry with all levels prepared before the first iteration (SiaUpT)
+  const SiaEntry* geo = nullptr;  // the launch geometry pick_launch chose
   size_t smem = 0;
   bool staged = false;
 };
@@ -1429,48 +1490,27 @@ void sia_split_free(svo_b200_ctx* ctx) {
 // footprints: the extra uncoalesced requests cost more L1 time than the DRAM latency they hide.
 constexpr size_t kSiaMinStageBytes = 20 * 1024;
 
-// Launch geometry for a batch of B pairs with at most max_feat features each.
-//   cluster == 1: one CTA per pair, 320 / 384 / 512 threads (one feature per thread up to 512, two up to 1024);
-//   cluster  > 1: (small batches) the pair's features are split over `cluster` CTAs of 96 threads.
-static size_t sia_shared_bytes(int threads, int cluster) {
-  if (cluster == 2) return sizeof(SiaSharedT<3, 2>);
-  if (cluster == 4) return sizeof(SiaSharedT<3, 4>);
-  if (cluster == 8) return sizeof(SiaSharedT<3, 8>);
-  if (threads == 160) return sizeof(SiaSharedT<5, 1>);
-  if (threads == 320) return sizeof(SiaSharedT<10, 1>);
-  if (threads == 384) return sizeof(SiaSharedT<12, 1>);
-  return sizeof(SiaSharedT<16, 1>);
-}
-
-static size_t sia_upfront_bytes(int cluster) {
-  if (cluster == 2) return sizeof(SiaUpT<3, 2>);
-  if (cluster == 4) return sizeof(SiaUpT<3, 4>);
-  return sizeof(SiaUpT<3, 8>);
-}
-
-// How many 4-CTA clusters of the (upfront or per-level) cluster kernel the device holds at once with `smem` bytes of dynamic
+// How many clusters of the (upfront or per-level) 4-CTA geometry `e` the device holds at once with `smem` bytes of dynamic
 // shared memory per CTA.  The general-camera instantiation stands for both: the plain-pinhole one has the same shared memory,
 // and at 96 threads per CTA registers do not limit residency.
-static int max_active_clusters(svo_b200_ctx* ctx, bool upfront, size_t smem, int& n) {
-  const int k = upfront ? 0 : 1;
+static int max_active_clusters(svo_b200_ctx* ctx, const SiaEntry& e, size_t smem, int& n) {
+  const int k = e.upfront ? 0 : 1;
   if (ctx->sia_occ_smem[k] != smem) {
-    const void* kern = upfront ? (const void*)sia_kernel<1, false, 96, 1, 4, true, true>
-                               : (const void*)sia_kernel<1, false, 96, 2, 4, true, false>;
-    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(e.kern[0], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(e.kern[0], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(4);
-    cfg.blockDim = dim3(96);
+    cfg.gridDim = dim3((unsigned)e.cluster);
+    cfg.blockDim = dim3((unsigned)e.threads);
     cfg.dynamicSmemBytes = smem;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 4;
+    attr[0].val.clusterDim.x = (unsigned)e.cluster;
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int c = 0;
-    SVO_CUDA_CHECK(ctx, cudaOccupancyMaxActiveClusters(&c, kern, &cfg));
+    SVO_CUDA_CHECK(ctx, cudaOccupancyMaxActiveClusters(&c, (const void*)e.kern[0], &cfg));
     ctx->sia_occ_smem[k] = smem;
     ctx->sia_occ_clusters[k] = c;
   }
@@ -1478,12 +1518,13 @@ static int max_active_clusters(svo_b200_ctx* ctx, bool upfront, size_t smem, int
   return 0;
 }
 
+// Launch geometry (an entry of kSiaEntries) for a batch of B pairs with at most max_feat features each: one CTA per pair,
+// or (small batches) the pair's features split over the CTAs of a thread-block cluster.
 // `fallback` (internal): 1 = the upfront clusters of this batch are not all resident at once, 2 = no cluster geometry is.
-static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& threads, int& fpt, int& cluster, bool& upfront,
-                       int& stage_cap, size_t& smem, int fallback = 0) {
+static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, const SiaEntry*& geo, int& stage_cap, size_t& smem,
+                       int fallback = 0) {
   if (max_feat > 1024)
     return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features per pair > 1024 (shared-memory patch cache)", max_feat);
-  cluster = 1;
   int want = ctx->sia_cluster;
   const bool auto_cluster = want < 0 && !ctx->xg_connected;
   if (ctx->xg_connected) {
@@ -1496,132 +1537,93 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, int& t
   // small batch (live streams, BASELINE configs[4]'s 32 pairs per GPU): spread each pair over 4 SMs while every CTA
   // still has an SM of its own (two cluster CTAs sharing an SM lose to one 320-thread CTA per pair)
   if (want < 0) want = (fallback < 2 && B * 4 <= ctx->sm_count) ? 4 : 1;
-  // full batches (more pairs than 2 per SM): 160 threads x 2 features, three CTAs per SM; in between, 320 x 1 with windows
-  // (with its state in shared memory and its loops rolled the 160 x 2 geometry also serves batches below two CTAs per SM,
-  // so the 320 x 1 geometry is left for > 304 features per pair, the multi-GPU split and explicit requests)
+  // full batches (more pairs than 2 per SM): the throughput geometry, 160 threads x 2 features, three CTAs per SM; in
+  // between, 320 x 1 with windows (with its state in shared memory and its loops rolled the throughput geometry also serves
+  // batches below two CTAs per SM, so the one-feature geometries are left for pairs beyond its slots, the multi-GPU split and
+  // explicit requests); otherwise the smallest one-CTA geometry whose slots hold the pair's features
   const bool fpt2 = ctx->sia_fpt != 1 && !ctx->xg_connected;
-  if (want > 1 && max_feat <= 96 * want && (want == 2 || want == 4 || want == 8)) cluster = want;
-  if (cluster > 1) {
-    fpt = 1;
-    threads = 96;
-  } else {
-    fpt = max_feat <= 512 ? 1 : 2;
-    threads = ((max_feat + fpt - 1) / fpt + 31) / 32 * 32;
-    // the kernels are instantiated for MAXT in {320, 384, 512}; launching exactly MAXT threads makes the
-    // slot count S = MAXT*FPT a compile-time constant (immediate shared-memory offsets)
-    threads = fpt == 1 ? (threads <= 320 ? 320 : threads <= 384 ? 384 : 512) : 512;
-    if (fpt2 && max_feat <= 304) { fpt = 2; threads = 160; }  // its shared arrays are allocated for 304 slots (kernel: SA)
-  }
-  const bool throughput_geom = cluster == 1 && fpt == 2 && threads == 160;
-  const int slots = throughput_geom ? 304 : threads * fpt;
-  size_t base = ((sia_shared_bytes(threads, cluster) + 15) & ~size_t(15)) + (size_t)3 * kPatchArea * slots * sizeof(float);
-  if (throughput_geom) base += (size_t)3 * slots * sizeof(double);  // xyz_ref of every feature (kernel: st_xyz)
+  auto first = [&](auto accept) -> const SiaEntry* {  // the first general-camera, per-level entry that holds max_feat
+    for (const SiaEntry& c : kSiaEntries)
+      if (c.general_camera && !c.upfront && max_feat <= c.cluster * c.slots && accept(c)) return &c;
+    return nullptr;
+  };
+  const SiaEntry* e = want > 1 ? first([&](const SiaEntry& c) { return c.cluster == want; }) : nullptr;
+  if (!e) e = first([&](const SiaEntry& c) { return c.cluster == 1 && (fpt2 || !c.throughput); });
   // cluster geometry with every CTA alone on its SM: one patch array set per level, everything pose independent prepared
-  // before the first iteration (the launch asks for the 4-CTA instantiation; 2 and 8 keep the per-level flow)
-  upfront = false;
-  if (cluster == 4 && ctx->sia_upfront != 0 && fallback == 0 && B * cluster <= ctx->sm_count && n_lvl >= 1 &&
-      n_lvl <= SVO_B200_MAX_LEVELS) {
-    const size_t base_up = ((sia_shared_bytes(threads, cluster) + 15) & ~size_t(15)) + ((sia_upfront_bytes(cluster) + 15) & ~size_t(15)) +
-                           (size_t)n_lvl * 3 * kPatchArea * slots * sizeof(float);
-    if (base_up + kSiaMinStageBytes + 1024 <= (size_t)ctx->max_smem_optin) {
-      upfront = true;
-      base = base_up;
-    }
-  }
-  // shared memory one CTA may use so that the intended number of CTAs stays resident per SM (228 KB per SM, 1 KB
-  // reserved per CTA)
-  const int resident = upfront ? 1 : cluster > 1 ? 2 : threads == 160 ? 3 : threads <= 384 ? 2 : 1;
+  // before the first iteration (only the 4-CTA geometry has an upfront instantiation; 2 and 8 keep the per-level flow)
+  const SiaEntry* up = sia_variant(*e, true, true);
+  if (up && ctx->sia_upfront != 0 && fallback == 0 && B * e->cluster <= ctx->sm_count && n_lvl >= 1 &&
+      n_lvl <= SVO_B200_MAX_LEVELS && up->fixed_bytes(n_lvl) + kSiaMinStageBytes + 1024 <= (size_t)ctx->max_smem_optin)
+    e = up;
+  const size_t base = e->fixed_bytes(e->upfront ? n_lvl : 1);
+  // shared memory one CTA may use so that the MINB CTAs the instantiation is compiled for stay resident per SM (228 KB per
+  // SM, 1 KB reserved per CTA)
   size_t budget = (size_t)ctx->max_smem_optin;
-  const size_t per_cta = (size_t)(228 * 1024) / resident - 1024;
+  const size_t per_cta = (size_t)(228 * 1024) / e->min_blocks - 1024;
   if (per_cta < budget) budget = per_cta;
   if (base + 1024 > budget)
     return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features need %zu B of shared memory", max_feat, base);
   // staging region: the coarse current-level images (TMA) or, at the fine levels, one 128-byte window per feature slot
   size_t cap = kSiaMinStageBytes;
-  const size_t win = (size_t)kWinBytes * slots;
+  const size_t win = (size_t)kWinBytes * e->slots;
   if (win > cap && base + win <= budget) cap = win;
   if (base + cap > budget) cap = (budget - base) & ~size_t(15);
+  geo = e;
   stage_cap = (int)cap;
   smem = base + cap;
   // The CTAs of a cluster run within one GPC, so whether all B clusters are resident at once depends on the GPC layout and
   // the shared memory per CTA; B * 4 <= #SMs does not imply it (an H100's 132 SMs sit in GPCs of different sizes).  A second
   // wave of clusters would double a small batch's latency: fall back to the per-level cluster flow (less shared memory per
   // CTA), and from there to one CTA per pair.  Explicit requests (svo_b200_sia_config / svo_b200_sia_upfront(1)) are kept.
-  if (auto_cluster && cluster == 4 && !(upfront && ctx->sia_upfront == 1)) {
+  if (auto_cluster && e->cluster == 4 && !(e->upfront && ctx->sia_upfront == 1)) {
     int n = 0;
-    if (int rc = max_active_clusters(ctx, upfront, smem, n)) return rc;
-    if (B > n) return pick_launch(ctx, B, max_feat, n_lvl, threads, fpt, cluster, upfront, stage_cap, smem, upfront ? 1 : 2);
+    if (int rc = max_active_clusters(ctx, *e, smem, n)) return rc;
+    if (B > n) return pick_launch(ctx, B, max_feat, n_lvl, geo, stage_cap, smem, e->upfront ? 1 : 2);
   }
   return 0;
 }
 
-// The template arguments of one sia_kernel instantiation (EVAL is launch_sia's), as a type launch_sia can report.
-template <int FPT_, int MAXT_, int MINB_, int CS_, bool CG_, bool UP_>
-struct SiaInst {
-  static constexpr int FPT = FPT_, MAXT = MAXT_, MINB = MINB_, CS = CS_;
-  static constexpr bool CG = CG_, UP = UP_;
-};
-
-template <bool EVAL>
-static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, int threads, int fpt, int cluster, bool upfront, size_t smem) {
-  auto go = [&](auto inst) -> int {
-    using I = decltype(inst);
-    using LAY = SiaLayout<I::FPT, I::MAXT, I::CS>;
-    const auto kern = sia_kernel<I::FPT, EVAL, I::MAXT, I::MINB, I::CS, I::CG, I::UP>;
-    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // ask for the full shared-memory carveout so that two CTAs of ~95 KB fit one SM
-    SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                             (int)cudaSharedmemCarveoutMaxShared));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(B * cluster));
-    cfg.blockDim = dim3((unsigned)threads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = cluster > 1 ? 1 : 0;
-    kt_begin(ctx);
-    SVO_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, kern, P));
-    kt_end(ctx);
-    ctx->launches++;
-    SVO_CUDA_CHECK(ctx, cudaGetLastError());
-    svo_b200_sia_launch& L = ctx->sia_last;  // what ran, for svo_b200_sia_last_launch
-    L = svo_b200_sia_launch{};
-    L.n_pairs = B; L.ctas_per_pair = I::CS; L.threads = threads; L.features_per_thread = I::FPT; L.min_blocks = I::MINB;
-    L.upfront = I::UP; L.general_camera = I::CG;
-    L.residuals_only = EVAL; L.stage_cap = P.stage_cap; L.smem_bytes = (int)smem; L.resident_clusters = ctx->sia_occ_clusters[0];
-    L.sm_count = ctx->sm_count;
-    L.min_level = EVAL ? P.eval_level : P.min_level;
-    L.max_level = EVAL ? P.eval_level : P.max_level;
-    for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l)
-      L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, LAY::WIN, LAY::SA) : -1;
-    ctx->sia_last_valid = true;
-    return 0;
-  };
-  // the undistorted pinhole gets its own instantiation of the geometries that carry the throughput / latency figures
-  // (the general-camera code also handles it; EVAL and the rarely used geometries are compiled once: with EVAL, CG = EVAL
-  // names the general-camera instantiation in both arms)
-  const bool plain = !EVAL && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE;
-  if (cluster == 2) return go(SiaInst<1, 96, 2, 2, true, false>{});
-  if (cluster == 4) {
-    if constexpr (!EVAL) {
-      if (upfront) return plain ? go(SiaInst<1, 96, 1, 4, false, true>{}) : go(SiaInst<1, 96, 1, 4, true, true>{});
-    }
-    return plain ? go(SiaInst<1, 96, 2, 4, EVAL, false>{}) : go(SiaInst<1, 96, 2, 4, true, false>{});
-  }
-  if (cluster == 8) return go(SiaInst<1, 96, 2, 8, true, false>{});
-  // <= 384 threads: cap registers so that two CTAs are resident per SM
-  if (fpt == 1) {
-    if (threads <= 320) return plain ? go(SiaInst<1, 320, 2, 1, EVAL, false>{}) : go(SiaInst<1, 320, 2, 1, true, false>{});
-    if (threads <= 384) return go(SiaInst<1, 384, 2, 1, true, false>{});
-    return go(SiaInst<1, 512, 1, 1, true, false>{});
-  }
-  if (threads == 160) return plain ? go(SiaInst<2, 160, 3, 1, EVAL, false>{}) : go(SiaInst<2, 160, 3, 1, true, false>{});
-  return go(SiaInst<2, 512, 1, 1, true, false>{});
+// Launches geometry `geo` (from pick_launch) and records the launch for svo_b200_sia_last_launch.  The undistorted pinhole
+// runs the geometry's plain-pinhole instantiation where it has one; the residual pass (eval) runs its general-camera,
+// per-level instantiation.
+static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, const SiaEntry& geo, size_t smem, bool eval) {
+  const bool plain = !eval && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE;
+  const SiaEntry* e = sia_variant(geo, !plain, geo.upfront && !eval);
+  if (!e) e = &geo;
+  const SiaKernel kern = e->kern[eval];
+  SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // ask for the full shared-memory carveout so that two CTAs of ~95 KB fit one SM
+  SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                           (int)cudaSharedmemCarveoutMaxShared));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(B * e->cluster));
+  cfg.blockDim = dim3((unsigned)e->threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = ctx->stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)e->cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = e->cluster > 1 ? 1 : 0;
+  kt_begin(ctx);
+  SVO_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, kern, P));
+  kt_end(ctx);
+  ctx->launches++;
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  svo_b200_sia_launch& L = ctx->sia_last;  // what ran, for svo_b200_sia_last_launch
+  L = svo_b200_sia_launch{};
+  L.n_pairs = B; L.ctas_per_pair = e->cluster; L.threads = e->threads; L.features_per_thread = e->fpt; L.min_blocks = e->min_blocks;
+  L.upfront = e->upfront; L.general_camera = e->general_camera;
+  L.residuals_only = eval; L.stage_cap = P.stage_cap; L.smem_bytes = (int)smem; L.resident_clusters = ctx->sia_occ_clusters[0];
+  L.sm_count = ctx->sm_count;
+  L.min_level = eval ? P.eval_level : P.min_level;
+  L.max_level = eval ? P.eval_level : P.max_level;
+  for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l)
+    L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, e->windows, e->slots) : -1;
+  ctx->sia_last_valid = true;
+  return 0;
 }
 
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
@@ -1764,12 +1766,8 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
     return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: NULL feature arrays");
   int rc = fill_common(ctx, st.P, ref[0], cam, opt);
   if (rc) return rc;
-  int stage_cap = 0;
-  rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.threads, st.fpt, st.cluster, st.upfront,
-                   stage_cap, st.smem);
+  rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.geo, st.P.stage_cap, st.smem);
   if (rc) return rc;
-  st.P.stage_cap = stage_cap;
-  st.P.slots = st.threads * st.fpt;
 
   // input staging: [jobs B][blobs]
   Carver cin;
@@ -1825,7 +1823,7 @@ int svo_b200_sia_batch_run(svo_b200_ctx* ctx) {
   if (!ctx || !ctx->sia || !ctx->sia->staged) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_run: nothing staged");
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
-  return launch_sia<false>(ctx, st.P, st.B, st.threads, st.fpt, st.cluster, st.upfront, st.smem);
+  return launch_sia(ctx, st.P, st.B, *st.geo, st.smem, false);
 }
 
 int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_out, double* H_out,
@@ -1911,7 +1909,7 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
   int rc = svo_b200_sia_batch_stage(ctx, 1, &ref, &cur, cam, &opt, T, off, px, f, point_pos, has_point, ref_pos);
   if (rc) return rc;
   SiaBatchState& st = *ctx->sia;
-  const size_t nslots = (size_t)st.P.slots * (size_t)st.cluster;
+  const size_t nslots = (size_t)st.geo->threads * st.geo->fpt * st.geo->cluster;
   Carver c;
   const size_t o_vin = c.take(N), o_rp = c.take(sizeof(float) * 16 * nslots),
                o_res = c.take(sizeof(float) * 16 * nslots), o_in = c.take(N),
@@ -1928,7 +1926,7 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
   st.P.Jres_out = reinterpret_cast<double*>(ds + o_j);
   st.P.chi2_out = reinterpret_cast<double*>(ds + o_c);
   st.P.n_meas_out = reinterpret_cast<long long*>(ds + o_n);
-  if ((rc = launch_sia<true>(ctx, st.P, 1, st.threads, st.fpt, st.cluster, false, st.smem))) return rc;
+  if ((rc = launch_sia(ctx, st.P, 1, *st.geo, st.smem, true))) return rc;
   double Tdummy[12];
   if ((rc = svo_b200_sia_batch_fetch(ctx, Tdummy, visible_io, H_out, nullptr))) return rc;
   if (ref_patch_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(ref_patch_out, ds + o_rp, sizeof(float) * 16 * (size_t)N, cudaMemcpyDeviceToHost));
