@@ -249,7 +249,9 @@ int svo_b200_align1d_batch(svo_b200_ctx* ctx, const svo_b200_frame* cur, int M, 
 
 /* M Matcher::findMatchDirect calls (after Point::getCloseViewObs chose the reference feature):
  * warp the 10x10 reference patch (getWarpMatrixAffine, getBestSearchLevel, warpAffine) and align.
- * ref_index[M] selects one of n_ref reference frames / poses. */
+ * ref_index[M] selects one of n_ref reference frames / poses; every ref_frames entry must be non-NULL.
+ * M == 0 returns 0 without reading the frames (n_ref may then be 0).  search_level_out, A_cur_ref_out
+ * and h_inv_out may be NULL. */
 typedef struct {
   int max_search_level; /* Config::nPyrLevels()-1 */
   int align_max_iter;   /* Matcher::Options::align_max_iter = 10 */

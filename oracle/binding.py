@@ -90,8 +90,8 @@ def cam_struct(cam) -> Camera:
     return Camera(cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, int(getattr(cam, "model", 0)), 0, d)
 
 
-def _level_ptrs(pyr):
-    arr = (C.c_void_p * len(pyr))()
+def _level_ptrs(pyr, n=None):
+    arr = (C.c_void_p * (len(pyr) if n is None else n))()  # entries past the pyramid's depth stay NULL
     for i, im in enumerate(pyr):
         assert im.dtype == np.uint8 and im.flags.c_contiguous
         arr[i] = im.ctypes.data
@@ -237,22 +237,34 @@ def ldlt6_solve(H, b):
     return x
 
 
-def align2d(cur_img, pwb, ref_patch, n_iter, px):
+ALIGN_EXITS = {1: "border_first", 2: "border", 3: "converged", 4: "max_iter", 5: "rollback", 6: "nan"}  # ORC_ALIGN_EXIT_*
+
+
+def align2d(cur_img, pwb, ref_patch, n_iter, px, want_exit=False):
+    """(converged, px); with want_exit, (converged, px, exit, n_iter_done) where exit is a name of ALIGN_EXITS."""
     px = c64(px).copy()
-    ok = lib().orc_align2d(_p(cur_img), cur_img.shape[1], cur_img.shape[0], cur_img.strides[0],
-                           _p(np.ascontiguousarray(pwb, np.uint8)), _p(np.ascontiguousarray(ref_patch, np.uint8)),
-                           n_iter, _p(px))
-    return bool(ok), px
+    a = (_p(cur_img), cur_img.shape[1], cur_img.shape[0], cur_img.strides[0], _p(np.ascontiguousarray(pwb, np.uint8)),
+         _p(np.ascontiguousarray(ref_patch, np.uint8)), int(n_iter), _p(px))
+    if not want_exit:
+        return bool(lib().orc_align2d(*a)), px
+    it, ex = C.c_int(0), C.c_int(0)
+    ok = lib().orc_align2d_ex(*a, C.byref(it), C.byref(ex))
+    return bool(ok), px, ALIGN_EXITS[ex.value], it.value
 
 
-def align1d(cur_img, direction, pwb, ref_patch, n_iter, px):
+def align1d(cur_img, direction, pwb, ref_patch, n_iter, px, want_exit=False):
+    """(converged, px, h_inv); with want_exit, (converged, px, h_inv, exit, n_iter_done)."""
     px = c64(px).copy()
     d = np.ascontiguousarray(direction, np.float32)
     h = C.c_double(0)
-    ok = lib().orc_align1d(_p(cur_img), cur_img.shape[1], cur_img.shape[0], cur_img.strides[0], _p(d),
-                           _p(np.ascontiguousarray(pwb, np.uint8)), _p(np.ascontiguousarray(ref_patch, np.uint8)),
-                           n_iter, _p(px), C.byref(h))
-    return bool(ok), px, h.value
+    a = (_p(cur_img), cur_img.shape[1], cur_img.shape[0], cur_img.strides[0], _p(d), _p(np.ascontiguousarray(pwb, np.uint8)),
+         _p(np.ascontiguousarray(ref_patch, np.uint8)), int(n_iter), _p(px), C.byref(h))
+    if not want_exit:
+        ok = lib().orc_align1d(*a)
+        return bool(ok), px, h.value
+    it, ex = C.c_int(0), C.c_int(0)
+    ok = lib().orc_align1d_ex(*a, C.byref(it), C.byref(ex))
+    return bool(ok), px, h.value, ALIGN_EXITS[ex.value], it.value
 
 
 def warp_matrix_affine(cam, px_ref, f_ref, depth, T_cur_ref, level_ref):
@@ -282,11 +294,17 @@ def depth_from_triangulation(T, f_ref, f_cur):
 
 def find_match_direct(ref_pyr, cur_pyr, cam, T_cur_ref, ref_px, ref_f, ref_level, ftr_type, ref_grad,
                       depth_ref, max_search_level, align_max_iter, px_cur):
-    rp, cols, rows = _level_ptrs(ref_pyr)
-    cp, _, _ = _level_ptrs(cur_pyr)
+    """The two pyramids share their level sizes but may differ in depth; the levels one of them lacks are passed as NULL
+    (the matcher reads ref_pyr[ref_level] and cur_pyr[search level] only)."""
+    n = max(len(ref_pyr), len(cur_pyr))
+    rp, _, _ = _level_ptrs(ref_pyr, n)
+    cp, _, _ = _level_ptrs(cur_pyr, n)
+    deeper = ref_pyr if len(ref_pyr) >= len(cur_pyr) else cur_pyr
+    cols = np.array([im.shape[1] for im in deeper], dtype=np.int32)
+    rows = np.array([im.shape[0] for im in deeper], dtype=np.int32)
     out = MatchResult()
     cs = cam_struct(cam)
-    lib().orc_find_match_direct(rp, cp, _p(cols), _p(rows), len(ref_pyr), C.byref(cs),
+    lib().orc_find_match_direct(rp, cp, _p(cols), _p(rows), n, C.byref(cs),
                                 _p(c64(T_cur_ref).reshape(12)), _p(c64(ref_px)), _p(c64(ref_f)),
                                 ref_level, ftr_type, _p(c64(ref_grad)), C.c_double(depth_ref),
                                 max_search_level, align_max_iter, _p(c64(px_cur)), C.byref(out))

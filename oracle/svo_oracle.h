@@ -99,6 +99,22 @@ int orc_align2d(const uint8_t* cur_img, int cols, int rows, int step,
 int orc_align1d(const uint8_t* cur_img, int cols, int rows, int step, const float* dir /*2*/,
                 const uint8_t* ref_patch_with_border, const uint8_t* ref_patch, int n_iter,
                 double* px_io /*2*/, double* h_inv_out);
+/* The same runs, also reporting how they ended (test instrumentation; the reference returns only the bool):
+ * n_iter_done = loop iterations run, the converging one included and a rolled-back one not;
+ * exit_reason = one of ORC_ALIGN_EXIT_*. */
+enum {
+  ORC_ALIGN_EXIT_BORDER_FIRST = 1, /* border test failed before the first step */
+  ORC_ALIGN_EXIT_BORDER = 2,       /* border test failed after at least one step */
+  ORC_ALIGN_EXIT_CONVERGED = 3,
+  ORC_ALIGN_EXIT_MAX_ITER = 4,     /* n_iter steps (also n_iter <= 0) */
+  ORC_ALIGN_EXIT_ROLLBACK = 5,     /* align1D only: chi2 rose, the last update was subtracted */
+  ORC_ALIGN_EXIT_NAN = 6           /* NaN after the border test: unreachable */
+};
+int orc_align2d_ex(const uint8_t* cur_img, int cols, int rows, int step, const uint8_t* ref_patch_with_border,
+                   const uint8_t* ref_patch, int n_iter, double* px_io, int* n_iter_done, int* exit_reason);
+int orc_align1d_ex(const uint8_t* cur_img, int cols, int rows, int step, const float* dir,
+                   const uint8_t* ref_patch_with_border, const uint8_t* ref_patch, int n_iter, double* px_io,
+                   double* h_inv_out, int* n_iter_done, int* exit_reason);
 
 /* ---- matcher warp (svo/src/matcher.cpp:33-133) ---- */
 void orc_get_warp_matrix_affine(const orc_camera* cam_ref, const orc_camera* cam_cur,

@@ -163,9 +163,13 @@ int svo_b200_find_match_direct(svo_b200_ctx* ctx, const svo_b200_frame* const* r
                                const int* ftr_type, const double* ref_grad, const double* point_pos,
                                double* px_cur_io, uint8_t* success_out, int* search_level_out,
                                double* A_cur_ref_out, double* h_inv_out) {
-  if (!ctx || !ref_frames || !ref_T_f_w || n_ref <= 0 || !cur || !cur_T_f_w || !cam || !opt || M < 0)
+  if (!ctx || !cur || !cur_T_f_w || !cam || !opt || M < 0)
     return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: bad arguments");
-  if (M == 0) return 0;
+  if (M == 0) return 0;  // no candidates: nothing to read, whatever the reference frames
+  if (!ref_frames || !ref_T_f_w || n_ref <= 0)
+    return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: no reference frames");
+  for (int r = 0; r < n_ref; ++r)
+    if (!ref_frames[r]) return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: ref_frames[%d] is NULL", r);
   if (!ref_index || !ref_px || !ref_f || !ref_level || !ftr_type || !ref_grad || !point_pos || !px_cur_io || !success_out)
     return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: NULL candidate arrays");
   for (int m = 0; m < M; ++m) {
