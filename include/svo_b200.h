@@ -103,6 +103,10 @@ int svo_b200_frame_upload(svo_b200_ctx* ctx, svo_b200_frame* frame, const uint8_
 int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* frame, const void* level0_dev);
 int svo_b200_frame_download_level(svo_b200_ctx* ctx, const svo_b200_frame* frame, int level,
                                   uint8_t* out);
+/* Every upload also writes a block-tiled copy of each level, which the alignment kernel gathers its footprints from.
+ * This copies it out, ceil(w/4) * ceil(h/4) * 16 bytes for a w x h level: block (bx, by) at byte 16 * (by * ceil(w/4) + bx)
+ * holds rows 4by..4by+3 of columns 4bx..4bx+3, four bytes per row; pixels outside the level are zero. */
+int svo_b200_frame_download_level_tiled(svo_b200_ctx* ctx, const svo_b200_frame* frame, int level, uint8_t* out);
 void svo_b200_frame_destroy(svo_b200_ctx* ctx, svo_b200_frame* frame);
 
 /* A pool = `count` frames of one geometry in ONE device slab (constant stride), so that a window of

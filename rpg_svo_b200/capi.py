@@ -147,6 +147,13 @@ class Frame:
         self.ctx._check(self.ctx.lib.svo_b200_frame_download_level(self.ctx.h, self.h, level, _p(out)))
         return out
 
+    def download_level_tiled(self, level: int) -> np.ndarray:
+        """The level's block-tiled copy as [ceil(h/4), ceil(w/4), 4 rows, 4 columns]."""
+        w, h = self.width >> level, self.height >> level
+        out = np.zeros(((h + 3) // 4, (w + 3) // 4, 4, 4), np.uint8)
+        self.ctx._check(self.ctx.lib.svo_b200_frame_download_level_tiled(self.ctx.h, self.h, level, _p(out)))
+        return out
+
     def destroy(self):
         if self.h and not getattr(self, "borrowed", False):
             self.ctx.lib.svo_b200_frame_destroy(self.ctx.h, self.h)

@@ -122,23 +122,50 @@ __global__ void half_sample_kernel(const uint8_t* __restrict__ in, int in_w, int
 // 128x16 tile of level 0 into the matching 64x8 / 32x4 / 16x2 / 8x1 tiles of levels 1..4 (as many as
 // the frame has), reading level 0 from HBM exactly once.  Same arithmetic as half_sample_kernel
 // (level l+1 = (a+b+c+d)/4 of level l), so the result is identical to the level-by-level build.
+// The kernel also writes the block-tiled copies (ctx.h) of the levels it reads or produces: whole 4x4 blocks from the
+// level-0 .. level-2 tiles, and the rows of level 3 / 4 blocks that fall into this tile.
 struct PyrGeom {
   int w[SVO_B200_MAX_LEVELS], h[SVO_B200_MAX_LEVELS];
   uint8_t* slab[SVO_B200_MAX_LEVELS];            // level l of frame i at slab[l] + i*stride[l]
   unsigned long long stride[SVO_B200_MAX_LEVELS];
+  uint8_t* tslab[SVO_B200_MAX_LEVELS];           // tiled copy of level l of frame i at tslab[l] + i*tstride[l]
+  unsigned long long tstride[SVO_B200_MAX_LEVELS];
   int n_levels;
   int tiles_x;
   unsigned avg_mask;  // bit l: level l is produced with the SSE2 rounding (avg of avg) instead of (a+b+c+d)/4
 };
+// Row word `w` of a block whose first column is x, of row y of a W x H level: pixels outside the level zeroed.
+__device__ __forceinline__ uint32_t tile_word(uint32_t w, int x, int y, int W, int H) {
+  if (y >= H || x >= W) return 0u;
+  return W - x >= 4 ? w : w & ((1u << (8 * (W - x))) - 1u);
+}
+// Rows r0..r0+n-1 (n = 1, 2 or 4) of block (bx, by) of the tiled copy of a W x H level from a shared tile `t` (pitch P, the
+// block's first column at c0 of tile row tr0): the words of rows r0.. are stored at word r0 of the block.  Blocks outside
+// the copy are skipped.
+template <int N>
+__device__ __forceinline__ void put_block_rows(uint8_t* tiled, int W, int H, int bx, int by, int r0, const uint8_t* t, int P,
+                                               int tr0, int c0) {
+  if (bx >= (W + 3) / 4 || by >= (H + 3) / 4) return;
+  uint32_t w[N];
+#pragma unroll
+  for (int r = 0; r < N; ++r)
+    w[r] = tile_word(*reinterpret_cast<const uint32_t*>(t + (tr0 + r) * P + c0), 4 * bx, 4 * by + r0 + r, W, H);
+  uint8_t* dst = tiled + ((size_t)by * ((W + 3) / 4) + bx) * 16 + 4 * r0;
+  if constexpr (N == 4) *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+  else if constexpr (N == 2) *reinterpret_cast<uint2*>(dst) = make_uint2(w[0], w[1]);
+  else *reinterpret_cast<uint32_t*>(dst) = w[0];
+}
 __global__ void __launch_bounds__(128) pyramid_fused_kernel(int first, PyrGeom g) {
   __shared__ __align__(16) uint8_t t0[16][128];
   __shared__ __align__(16) uint8_t t1[8][64];
   __shared__ __align__(16) uint8_t t2[4][32];
   __shared__ __align__(16) uint8_t t3[2][16];
+  __shared__ __align__(16) uint8_t t4[1][8];
   const size_t fi = (size_t)(first + blockIdx.y);
   const int tx = blockIdx.x % g.tiles_x, ty = blockIdx.x / g.tiles_x;
   const int t = threadIdx.x;
   const int W0 = g.w[0], H0 = g.h[0];
+  auto tiled = [&](int l) { return g.tslab[l] + fi * g.tstride[l]; };
   {  // level-0 tile -> shared (16 B per thread)
     const int r = t >> 3, c = (t & 7) * 16;
     const int y = ty * 16 + r, x = tx * 128 + c;
@@ -157,6 +184,8 @@ __global__ void __launch_bounds__(128) pyramid_fused_kernel(int first, PyrGeom g
     *reinterpret_cast<uint4*>(&t0[r][c]) = v;
   }
   __syncthreads();
+  // level 0 tiled: 4 x 32 blocks, one per thread
+  put_block_rows<4>(tiled(0), W0, H0, tx * 32 + (t & 31), ty * 4 + (t >> 5), 0, &t0[0][0], 128, 4 * (t >> 5), 4 * (t & 31));
   if (g.n_levels > 1) {  // level 1: 8 x 64, four pixels per thread
     const int r = t >> 4, c = (t & 15) * 4;
     const uint2 a = *reinterpret_cast<const uint2*>(&t0[2 * r][2 * c]);
@@ -175,6 +204,8 @@ __global__ void __launch_bounds__(128) pyramid_fused_kernel(int first, PyrGeom g
     }
   }
   __syncthreads();
+  if (g.n_levels > 1 && t < 32)  // level 1 tiled: 2 x 16 blocks
+    put_block_rows<4>(tiled(1), g.w[1], g.h[1], tx * 16 + (t & 15), ty * 2 + (t >> 4), 0, &t1[0][0], 64, 4 * (t >> 4), 4 * (t & 15));
   if (g.n_levels > 2) {  // level 2: 4 x 32
     const int r = t >> 5, c = t & 31;
     const uint8_t o = (uint8_t)half1(t1[2 * r][2 * c], t1[2 * r][2 * c + 1], t1[2 * r + 1][2 * c], t1[2 * r + 1][2 * c + 1],
@@ -184,6 +215,8 @@ __global__ void __launch_bounds__(128) pyramid_fused_kernel(int first, PyrGeom g
     if (y < g.h[2] && x < g.w[2]) g.slab[2][fi * g.stride[2] + (size_t)y * g.w[2] + x] = o;
   }
   __syncthreads();
+  if (g.n_levels > 2 && t < 8)  // level 2 tiled: 1 x 8 blocks
+    put_block_rows<4>(tiled(2), g.w[2], g.h[2], tx * 8 + t, ty, 0, &t2[0][0], 32, 0, 4 * t);
   if (g.n_levels > 3 && t < 32) {  // level 3: 2 x 16
     const int r = t >> 4, c = t & 15;
     const uint8_t o = (uint8_t)half1(t2[2 * r][2 * c], t2[2 * r][2 * c + 1], t2[2 * r + 1][2 * c], t2[2 * r + 1][2 * c + 1],
@@ -193,33 +226,44 @@ __global__ void __launch_bounds__(128) pyramid_fused_kernel(int first, PyrGeom g
     if (y < g.h[3] && x < g.w[3]) g.slab[3][fi * g.stride[3] + (size_t)y * g.w[3] + x] = o;
   }
   __syncthreads();
+  if (g.n_levels > 3 && t < 4)  // level 3 tiled: rows 2ty, 2ty+1 of 4 blocks
+    put_block_rows<2>(tiled(3), g.w[3], g.h[3], tx * 4 + t, ty >> 1, 2 * (ty & 1), &t3[0][0], 16, 0, 4 * t);
   if (g.n_levels > 4 && t < 8) {  // level 4: 1 x 8
     const int y = ty, x = tx * 8 + t;
-    if (y < g.h[4] && x < g.w[4])
-      g.slab[4][fi * g.stride[4] + (size_t)y * g.w[4] + x] =
-          (uint8_t)half1(t3[0][2 * t], t3[0][2 * t + 1], t3[1][2 * t], t3[1][2 * t + 1], (g.avg_mask >> 4) & 1u);
+    const uint8_t o = (uint8_t)half1(t3[0][2 * t], t3[0][2 * t + 1], t3[1][2 * t], t3[1][2 * t + 1], (g.avg_mask >> 4) & 1u);
+    t4[0][t] = o;
+    if (y < g.h[4] && x < g.w[4]) g.slab[4][fi * g.stride[4] + (size_t)y * g.w[4] + x] = o;
   }
+  __syncthreads();
+  if (g.n_levels > 4 && t < 2)  // level 4 tiled: row ty of 2 blocks
+    put_block_rows<1>(tiled(4), g.w[4], g.h[4], tx * 2 + t, ty >> 2, ty & 3, &t4[0][0], 8, 0, 4 * t);
 }
 
 
 // Level 0 -> level 1 for a batch of frames as a pure streaming kernel: 94 % of the pyramid's bytes move
 // here, so it is written against the HBM roofline -- a persistent grid (a few CTAs per SM), each work
 // item = 16 level-0 pixels of two consecutive rows (2 x 128-bit loads) -> 8 level-1 pixels (one 64-bit
-// store); the 2x2 reductions are formed SIMD-in-register (scalar rule: two 16-bit lanes per word; SSE2 rule: two
-// __vavgu4).  Requires W0 % 16 == 0.
+// store), plus those two rows of the four level-0 blocks they cover in the tiled copy t0 (four 64-bit stores).
+// The 2x2 reductions are formed SIMD-in-register (scalar rule: two 16-bit lanes per word; SSE2 rule: two __vavgu4).  An
+// odd last level-0 row is tiled alone.  Requires W0 % 16 == 0.
 __global__ void __launch_bounds__(256) pyramid_l0_l1_stream_kernel(const uint8_t* __restrict__ l0, size_t stride0,
-                                                                   uint8_t* __restrict__ l1, size_t stride1, int first,
-                                                                   int count, int W0, int H1, int avg) {
-  const int items_x = W0 >> 4, W1 = W0 >> 1;
-  const long long per_frame = (long long)items_x * H1, total = per_frame * count;
+                                                                   uint8_t* __restrict__ l1, size_t stride1,
+                                                                   uint8_t* __restrict__ t0, size_t tstride0, int first,
+                                                                   int count, int W0, int H0, int avg) {
+  const int items_x = W0 >> 4, W1 = W0 >> 1, H1 = H0 >> 1, BW0 = W0 >> 2;
+  const long long per_frame = (long long)items_x * ((H0 + 1) >> 1), total = per_frame * count;
   for (long long it = (long long)blockIdx.x * blockDim.x + threadIdx.x; it < total; it += (long long)gridDim.x * blockDim.x) {
     const int fr = (int)(it / per_frame);
     const int rem = (int)(it - (long long)fr * per_frame);
     const int y = rem / items_x, ix = rem - y * items_x;
     const uint8_t* src = l0 + (size_t)(first + fr) * stride0 + (size_t)(2 * y) * W0 + 16 * ix;
     const uint4 a = __ldg(reinterpret_cast<const uint4*>(src));
-    const uint4 b = __ldg(reinterpret_cast<const uint4*>(src + W0));
+    const uint4 b = y < H1 ? __ldg(reinterpret_cast<const uint4*>(src + W0)) : make_uint4(0u, 0u, 0u, 0u);
     const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
+    uint2* tl = reinterpret_cast<uint2*>(t0 + (size_t)(first + fr) * tstride0 + ((size_t)(y >> 1) * BW0 + 4 * ix) * 16 + 8 * (y & 1));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tl[2 * k] = make_uint2(aw[k], bw[k]);
+    if (y >= H1) continue;
     uint32_t o[2] = {0u, 0u};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -231,13 +275,71 @@ __global__ void __launch_bounds__(256) pyramid_l0_l1_stream_kernel(const uint8_t
   }
 }
 
+// Block-tiled copy of levels [first_level, first_level + gridDim.y) of `count` frames, level l of frame i at lvl[l] +
+// i * stride[l], its copy at tl[l] + i * tstride[l]: one thread per 4x4 block, zero outside the level.  Tiles the levels no pyramid kernel tiles: levels
+// uploaded from the host, and levels below the fused kernel's.
+struct TileGeom {
+  uint8_t* lvl[SVO_B200_MAX_LEVELS];
+  unsigned long long stride[SVO_B200_MAX_LEVELS];
+  uint8_t* tl[SVO_B200_MAX_LEVELS];
+  unsigned long long tstride[SVO_B200_MAX_LEVELS];
+  int w[SVO_B200_MAX_LEVELS], h[SVO_B200_MAX_LEVELS];
+};
+__global__ void __launch_bounds__(256) tile_levels_kernel(TileGeom g, int first_level, int count) {
+  const int l = first_level + (int)blockIdx.y;
+  const int W = g.w[l], H = g.h[l], BW = (W + 3) >> 2;
+  const long long per_frame = (long long)BW * ((H + 3) >> 2), total = per_frame * count;
+  for (long long it = (long long)blockIdx.x * blockDim.x + threadIdx.x; it < total; it += (long long)gridDim.x * blockDim.x) {
+    const int fr = (int)(it / per_frame);
+    const int b = (int)(it - (long long)fr * per_frame);
+    const int by = b / BW, bx = b - by * BW;
+    const uint8_t* src = g.lvl[l] + (size_t)fr * g.stride[l];
+    uint32_t w[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int y = 4 * by + r, x = 4 * bx;
+      w[r] = 0u;
+      if (y < H) {
+        const uint8_t* p = src + (size_t)y * W + x;
+        if ((W & 3) == 0) {
+          w[r] = *reinterpret_cast<const uint32_t*>(p);
+        } else {
+          for (int k = 0; k < 4 && x + k < W; ++k) w[r] |= (uint32_t)p[k] << (8 * k);
+        }
+      }
+    }
+    reinterpret_cast<uint4*>(g.tl[l] + (size_t)fr * g.tstride[l])[b] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+// tile_levels_kernel over levels [from, to) of `count` frames, level l of frame i at lvl[l] + i * stride[l], its copy at
+// tl[l] + i * tstride[l] (strides: nullptr for one frame)
+static int tile_levels(svo_b200_ctx* ctx, uint8_t* const* lvl, const size_t* stride, uint8_t* const* tl, const size_t* tstride,
+                       const int* w, const int* h, int from, int to, int count) {
+  if (from >= to) return 0;
+  TileGeom g;
+  memset(&g, 0, sizeof(g));
+  for (int l = from; l < to; ++l) {
+    g.lvl[l] = lvl[l]; g.stride[l] = stride ? stride[l] : 0; g.tl[l] = tl[l]; g.tstride[l] = tstride ? tstride[l] : 0;
+    g.w[l] = w[l]; g.h[l] = h[l];
+  }
+  const long long n = (long long)((w[from] + 3) / 4) * ((h[from] + 3) / 4) * count;  // blocks of the largest level
+  long long blocks = (n + 255) / 256;
+  if (blocks > ctx->sm_count * 8LL) blocks = ctx->sm_count * 8LL;
+  tile_levels_kernel<<<dim3((unsigned)blocks, (unsigned)(to - from)), 256, 0, ctx->stream>>>(g, from, count);
+  ctx->launches++;
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  return 0;
+}
+
 // does producing a level from a source level of width `src_w` use vikit's SSE2 rounding?  (x86 rule: width % 16 == 0;
 // cv::Mat buffers are always 16-byte aligned)
 static inline int pyr_avg(const svo_b200_ctx* ctx, int src_w) {
   return ctx->pyramid_rule == SVO_B200_PYR_X86 && (src_w % 16) == 0;
 }
 
-static int build_levels(svo_b200_ctx* ctx, svo_b200_frame* fr, int from_level, bool timed = true) {
+// Levels [from_level, n_levels) of one frame from the level above, then the tiled copies of levels [tile_from, n_levels).
+static int build_levels(svo_b200_ctx* ctx, svo_b200_frame* fr, int from_level, int tile_from, bool timed = true) {
   if (timed) kt_begin(ctx);
   for (int l = from_level; l < fr->n_levels; ++l) {
     const int total = ((fr->w[l] + 3) / 4) * fr->h[l];
@@ -249,8 +351,9 @@ static int build_levels(svo_b200_ctx* ctx, svo_b200_frame* fr, int from_level, b
                                                             fr->lvl(l), fr->w[l], fr->h[l], pyr_avg(ctx, fr->w[l - 1]));
     ctx->launches++;
   }
-  if (timed) kt_end(ctx);
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  if (int rc = tile_levels(ctx, fr->lv, nullptr, fr->tv, nullptr, fr->w, fr->h, tile_from, fr->n_levels, 1)) return rc;
+  if (timed) kt_end(ctx);
   return 0;
 }
 
@@ -349,7 +452,7 @@ int svo_b200_frame_create(svo_b200_ctx* ctx, int width, int height, int n_levels
       return set_err(ctx, SVO_B200_EINVAL, "frame_create: level %d is empty", l);
     }
     fr->off[l] = off;
-    off += ((size_t)fr->w[l] * fr->h[l] + 255 + 16) / 256 * 256;  // +16: kernels may read one word past
+    off += row_major_bytes(fr->w[l], fr->h[l]) + (tiled_bytes(fr->w[l], fr->h[l]) + 255) / 256 * 256;
   }
   fr->bytes = off;
   cudaError_t e = cudaMalloc((void**)&fr->base, fr->bytes);
@@ -357,7 +460,10 @@ int svo_b200_frame_create(svo_b200_ctx* ctx, int width, int height, int n_levels
     delete fr;
     return set_err(ctx, SVO_B200_ENOMEM, "frame_create: cudaMalloc(%zu): %s", off, cudaGetErrorString(e));
   }
-  for (int l = 0; l < n_levels; ++l) fr->lv[l] = fr->base + fr->off[l];
+  for (int l = 0; l < n_levels; ++l) {
+    fr->lv[l] = fr->base + fr->off[l];
+    fr->tv[l] = fr->lv[l] + row_major_bytes(fr->w[l], fr->h[l]);
+  }
   cudaMemsetAsync(fr->base, 0, fr->bytes, ctx->stream);
   *frame_out = fr;
   return 0;
@@ -372,7 +478,7 @@ int svo_b200_frame_upload(svo_b200_ctx* ctx, svo_b200_frame* fr, const uint8_t* 
     SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(fr->lvl(l), levels[l], (size_t)fr->w[l] * fr->h[l],
                                         cudaMemcpyHostToDevice, ctx->stream));
   }
-  return build_levels(ctx, fr, n_given);
+  return build_levels(ctx, fr, n_given, 0);
 }
 
 int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* fr, const void* level0_dev) {
@@ -380,7 +486,17 @@ int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* fr, const vo
   cudaSetDevice(ctx->device);
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(fr->lvl(0), level0_dev, (size_t)fr->w[0] * fr->h[0],
                                       cudaMemcpyDeviceToDevice, ctx->stream));
-  return build_levels(ctx, fr, 1);
+  return build_levels(ctx, fr, 1, 0);
+}
+
+int svo_b200_frame_download_level_tiled(svo_b200_ctx* ctx, const svo_b200_frame* fr, int level, uint8_t* out) {
+  if (!ctx || !fr || !out || level < 0 || level >= fr->n_levels)
+    return set_err(ctx, SVO_B200_EINVAL, "frame_download_level_tiled: bad arguments");
+  cudaSetDevice(ctx->device);
+  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(out, fr->tv[level],
+                                      tiled_bytes(fr->w[level], fr->h[level]), cudaMemcpyDeviceToHost, ctx->stream));
+  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  return 0;
 }
 
 int svo_b200_frame_download_level(svo_b200_ctx* ctx, const svo_b200_frame* fr, int level, uint8_t* out) {
@@ -427,16 +543,28 @@ int svo_b200_frame_pool_create(svo_b200_ctx* ctx, int width, int height, int n_l
     slab_off[l] = total;
     total += pool->stride[l] * (size_t)count + 256;  // slack: kernels fetch aligned words around footprints
   }
+  size_t tslab_off[SVO_B200_MAX_LEVELS];
+  for (int l = 0; l < n_levels; ++l) {
+    pool->tstride[l] = (tiled_bytes(proto.w[l], proto.h[l]) + 255) / 256 * 256;
+    tslab_off[l] = total;
+    total += pool->tstride[l] * (size_t)count;
+  }
   cudaError_t e = cudaMalloc((void**)&pool->mem, total);
   if (e != cudaSuccess) {
     delete pool;
     return set_err(ctx, SVO_B200_ENOMEM, "frame_pool_create: cudaMalloc(%zu): %s", total, cudaGetErrorString(e));
   }
   cudaMemsetAsync(pool->mem, 0, total, ctx->stream);
-  for (int l = 0; l < n_levels; ++l) pool->slab[l] = pool->mem + slab_off[l];
+  for (int l = 0; l < n_levels; ++l) {
+    pool->slab[l] = pool->mem + slab_off[l];
+    pool->tslab[l] = pool->mem + tslab_off[l];
+  }
   pool->frames.assign(count, proto);
   for (int i = 0; i < count; ++i)
-    for (int l = 0; l < n_levels; ++l) pool->frames[i].lv[l] = pool->slab[l] + (size_t)i * pool->stride[l];
+    for (int l = 0; l < n_levels; ++l) {
+      pool->frames[i].lv[l] = pool->slab[l] + (size_t)i * pool->stride[l];
+      pool->frames[i].tv[l] = pool->tslab[l] + (size_t)i * pool->tstride[l];
+    }
   *pool_out = pool;
   return 0;
 }
@@ -461,18 +589,21 @@ int svo_b200_frame_pool_upload(svo_b200_ctx* ctx, svo_b200_frame_pool* pool, int
     SVO_CUDA_CHECK(ctx, cudaMemcpy2DAsync(dst, pool->stride[0], level0_host, host_stride_bytes, img, (size_t)count,
                                           cudaMemcpyHostToDevice, ctx->stream));
   }
+  kt_begin(ctx);
+  int tiled = 0;  // levels [0, tiled) get their tiled copies from the pyramid kernels
   if (f0.n_levels > 1) {
     // level 0 -> 1 with the streaming kernel when the width allows 128-bit rows, then levels 2.. from
     // level 1 with the fused tile kernel (base level shifted by one); otherwise everything from level 0.
     const bool stream01 = (f0.w[0] % 16) == 0;
     const int base = stream01 ? 1 : 0;
-    kt_begin(ctx);
     if (stream01) {
       const int blocks = ctx->sm_count * 8;
       pyramid_l0_l1_stream_kernel<<<blocks, 256, 0, ctx->stream>>>(pool->slab[0], pool->stride[0], pool->slab[1],
-                                                                   pool->stride[1], first, count, f0.w[0], f0.h[1],
+                                                                   pool->stride[1], pool->tslab[0], pool->tstride[0], first,
+                                                                   count, f0.w[0], f0.h[0],
                                                                    pyr_avg(ctx, f0.w[0]));
       ctx->launches++;
+      tiled = 1;
     }
     const int n_sub = f0.n_levels - base;  // levels seen by the fused kernel, its level 0 = our level `base`
     if (n_sub > 1) {
@@ -481,6 +612,7 @@ int svo_b200_frame_pool_upload(svo_b200_ctx* ctx, svo_b200_frame_pool* pool, int
       g.n_levels = n_sub < 5 ? n_sub : 5;
       for (int l = 0; l < n_sub; ++l) {
         g.w[l] = f0.w[base + l]; g.h[l] = f0.h[base + l]; g.slab[l] = pool->slab[base + l]; g.stride[l] = pool->stride[base + l];
+        g.tslab[l] = pool->tslab[base + l]; g.tstride[l] = pool->tstride[base + l];
       }
       for (int l = 1; l < g.n_levels; ++l)
         if (pyr_avg(ctx, g.w[l - 1])) g.avg_mask |= 1u << l;
@@ -492,14 +624,21 @@ int svo_b200_frame_pool_upload(svo_b200_ctx* ctx, svo_b200_frame_pool* pool, int
         pyramid_fused_kernel<<<grid, 128, 0, ctx->stream>>>(first + done, g);
         ctx->launches++;
       }
+      tiled = base + g.n_levels;
     }
     SVO_CUDA_CHECK(ctx, cudaGetLastError());
     for (int i = 0; i < count && f0.n_levels > base + 5; ++i) {  // deeper levels: plain per-level kernel
-      int rc = build_levels(ctx, &pool->frames[first + i], base + 5, false);
+      int rc = build_levels(ctx, &pool->frames[first + i], base + 5, f0.n_levels, false);
       if (rc) return rc;
     }
-    kt_end(ctx);
   }
+  uint8_t *lv[SVO_B200_MAX_LEVELS], *tv[SVO_B200_MAX_LEVELS];
+  for (int l = 0; l < f0.n_levels; ++l) {
+    lv[l] = pool->slab[l] + (size_t)first * pool->stride[l];
+    tv[l] = pool->tslab[l] + (size_t)first * pool->tstride[l];
+  }
+  if (int rc = tile_levels(ctx, lv, pool->stride, tv, pool->tstride, f0.w, f0.h, tiled, f0.n_levels, count)) return rc;
+  kt_end(ctx);
   return 0;
 }
 

@@ -63,6 +63,10 @@ constexpr int kWinBytes = kWinRows * 16;  // 128 B per feature slot
 struct SiaJob {  // one frame pair; array lives in device memory
   const uint8_t* ref_lvl[SVO_B200_MAX_LEVELS];
   const uint8_t* cur_lvl[SVO_B200_MAX_LEVELS];
+  // block-tiled copies of the levels (ctx.h).  Pointers of their own, not an offset from the row-major level: a frame pool
+  // keeps its copies apart so that its level-0 images stay contiguous (one flat upload per window).
+  const uint8_t* ref_tl[SVO_B200_MAX_LEVELS];
+  const uint8_t* cur_tl[SVO_B200_MAX_LEVELS];
   const uint8_t* blob;  // packed features: px[np*2] f[np*3] pos[np*3] (f64) then has_point[np] (u8)
   int n_feat, n_pad;
   int feat_off;  // offset of this pair in visible_out
@@ -145,6 +149,7 @@ struct SiaSharedT {
   unsigned xg_seq;     // feature split over GPUs: exchanges completed (warp 0) ...
   unsigned xg_failed;  // ... and "an exchange timed out" (must directly follow xg_seq)
   alignas(16) double pub[12];  // CS == 1: the pose (R row-major, t) warp 0 publishes after its Gauss-Newton tail
+  const uint4* cur_tl;         // tiled copy of the current image of the running level (throughput geometry)
   int pub_done, pub_slow;
 #if SVO_SIA_DEBUG
   long long tkx[4];
@@ -204,6 +209,75 @@ __device__ __forceinline__ void fetch12(const uint8_t* base, int off, uint32_t& 
                  w2 = ld_word<SMEM>(base, a + 8);
   lo = __funnelshift_r(w0, w1, sh);
   hi = __funnelshift_r(w1, w2, sh);
+}
+
+// Footprint gathers from the block-tiled copy of a level (ctx.h: 16-byte blocks of 4x4 pixels, one 32-bit
+// word per row, `bw` blocks per block-row).  A column of blocks yields a sequence of row words q = 0, 1, ... from the block-row
+// of the footprint's first row y0; row r of the footprint is word q = r + (y0 & 3), picked by two select stages (rotate by
+// 2, then by 1).  The same funnel shifts as the row-major fetches then give the same bytes, so the pixel values and everything
+// computed from them are unchanged.
+template <int N>
+__device__ __forceinline__ void rotate_rows(const uint32_t (&q)[N + 3], int s, uint32_t (&out)[N]) {
+  uint32_t v[N + 1];
+#pragma unroll
+  for (int i = 0; i <= N; ++i) v[i] = (s & 2) ? q[i + 2] : q[i];
+#pragma unroll
+  for (int r = 0; r < N; ++r) out[r] = (s & 1) ? v[r + 1] : v[r];
+}
+// 5x5: rows y0..y0+4, columns x0..x0+4 lie in exactly 2x2 blocks -- four loads.  lo[r] = columns x0..x0+3 of row y0+r, the
+// low byte of hi[r] = column x0+4 (as fetch8).  Of the 8 row words of a block column the footprint needs words s..s+4
+// (s = y0 & 3), so words (s & 2) .. (s & 2) + 5 are loaded -- one whole block and the adjacent half of the other, 6 registers
+// instead of 8 (the residual pass runs at the register limit) -- and the first select stage of rotate_rows is done by the
+// addresses.
+__device__ __forceinline__ void fetch5x5_tiled(const uint4* tl, int bw, int x0, int y0, uint32_t (&lo)[5], uint32_t (&hi)[5]) {
+  const uint4* b = tl + (y0 >> 2) * bw + (x0 >> 2);
+  const bool s2 = (y0 & 2) != 0, s1 = (y0 & 1) != 0;
+  // s2: the bottom block whole, words 2, 3 of the top one; else the top block whole, words 0, 1 of the bottom one
+  const uint4* pw = s2 ? b + bw : b;
+  const uint2* ph = reinterpret_cast<const uint2*>(s2 ? b : b + bw) + (s2 ? 1 : 0);
+  const uint4 l4 = __ldg(pw), r4 = __ldg(pw + 1);
+  const uint2 l2 = __ldg(ph), r2 = __ldg(ph + 2);
+  const uint32_t vl[6] = {s2 ? l2.x : l4.x, s2 ? l2.y : l4.y, s2 ? l4.x : l4.z, s2 ? l4.y : l4.w, s2 ? l4.z : l2.x, s2 ? l4.w : l2.y};
+  const uint32_t vr[6] = {s2 ? r2.x : r4.x, s2 ? r2.y : r4.y, s2 ? r4.x : r4.z, s2 ? r4.y : r4.w, s2 ? r4.z : r2.x, s2 ? r4.w : r2.y};
+  uint32_t wl[5], wr[5];
+#pragma unroll
+  for (int r = 0; r < 5; ++r) {
+    wl[r] = s1 ? vl[r + 1] : vl[r];
+    wr[r] = s1 ? vr[r + 1] : vr[r];
+  }
+  const unsigned sh = (unsigned)(x0 & 3) * 8u;
+#pragma unroll
+  for (int r = 0; r < 5; ++r) {
+    lo[r] = __funnelshift_r(wl[r], wr[r], sh);
+    hi[r] = wr[r] >> sh;
+  }
+}
+// 7x7: rows y0..y0+6, columns x0..x0+6 lie in 2 or 3 blocks per axis (6.25 loads on average).  Walked one block-row at a time,
+// each block-row's words funnel-shifted into two words per row at once, so that the raw words of a block-row need not stay live.  lo[r] = columns
+// x0..x0+3 of row y0+r, bytes 0..2 of hi[r] = columns x0+4..x0+6 (as fetch7_g64).  The third block column / block-row is
+// loaded only when the footprint reaches into it (always inside the level when the footprint is).
+__device__ __forceinline__ void fetch7x7_tiled(const uint4* tl, int bw, int x0, int y0, uint32_t (&lo)[7], uint32_t (&hi)[7]) {
+  const uint4* b = tl + (y0 >> 2) * bw + (x0 >> 2);
+  const int s = y0 & 3;
+  const bool col3 = (x0 & 3) >= 2;
+  const unsigned sh = (unsigned)(x0 & 3) * 8u;
+  uint32_t ql[10], qh[10];  // funnel-shifted words of rows q = 0..9 from block-row y0 >> 2 (rows s..s+6 are the footprint's)
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const bool load = j < 2 || s >= 2;
+    const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+    const uint4 x = load ? __ldg(b + j * bw) : zero, y = load ? __ldg(b + j * bw + 1) : zero;
+    const uint4 z = load && col3 ? __ldg(b + j * bw + 2) : zero;
+    const uint32_t xw[4] = {x.x, x.y, x.z, x.w}, yw[4] = {y.x, y.y, y.z, y.w}, zw[4] = {z.x, z.y, z.z, z.w};
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      if (4 * j + w >= 10) break;
+      ql[4 * j + w] = __funnelshift_r(xw[w], yw[w], sh);
+      qh[4 * j + w] = __funnelshift_r(yw[w], zw[w], sh);
+    }
+  }
+  rotate_rows<7>(ql, s, lo);
+  rotate_rows<7>(qh, s, hi);
 }
 
 // Element k of a per-feature register array, read with compile-time indices only: in a loop over the thread's features that
@@ -613,6 +687,11 @@ struct SiaInst {
   // ~20 KB, which matters with three CTAs in different phases sharing one instruction cache.
   static constexpr bool WIN = !SS;  // per-feature cp.async windows of the current image exist in this instantiation
   static constexpr bool XG = CS == 1 && !SS;  // multi-GPU feature split (svo_b200_sia_split_*) compiled in
+  // The throughput geometry gathers from global memory -- the reference footprints of every level, the current footprints of
+  // the levels not staged whole -- from the block-tiled copy of the level (two 16-byte and two 8-byte loads per 5x5 footprint
+  // instead of ten 32-bit loads, 6.25 16-byte loads instead of ~12 8-byte ones per 7x7 one).  The other geometries stage windows or whole images and keep the
+  // row-major gathers.
+  static constexpr bool TL = SS;
   using SH = SiaSharedT<NWC, CS>;
   using UPT = SiaUpT<NWC, CS>;
   // dynamic shared memory: control block (SH, then UPT when UP), patch array sets, xyz_ref (SS), staging region
@@ -652,6 +731,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   constexpr int SA = G::SA;
   constexpr bool WIN = G::WIN;
   constexpr bool XG = G::XG;
+  constexpr bool TL = G::TL;
   UPT& up = *reinterpret_cast<UPT*>(smem_raw + G::kShBytes);  // only touched when UP
   const int n_lvl_bufs = UP ? (P.max_level - P.min_level + 1) : 1;  // patch array sets (one per level when UP)
   // the regions in the order of SiaInst::fixed_bytes (pointer steps in the regions' element types: stepping in bytes
@@ -891,6 +971,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     const float scale = 1.0f / (float)(1 << level);
     const uint8_t* ref_img = job.ref_lvl[level];
     const uint8_t* cur_img = job.cur_lvl[level];
+    const uint4* ref_tl = reinterpret_cast<const uint4*>(job.ref_tl[level]);
 #pragma unroll(SS ? 1 : FPT)
     for (int k = 0; k < FPT; ++k) {
       if constexpr (!SS) m_sxx[k] = m_sxy[k] = m_syy[k] = 0.0;
@@ -907,8 +988,12 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       uint32_t rlo[7], rhi[7];
       if (ok) {
         vis_mask |= 1u << k;
+        if constexpr (TL) {
+          fetch7x7_tiled(ref_tl, (W + 3) >> 2, ui - 3, vi - 3, rlo, rhi);
+        } else {
 #pragma unroll
-        for (int r = 0; r < 7; ++r) fetch7_g64(ref_img, (vi - 3 + r) * W + (ui - 3), rlo[r], rhi[r]);
+          for (int r = 0; r < 7; ++r) fetch7_g64(ref_img, (vi - 3 + r) * W + (ui - 3), rlo[r], rhi[r]);
+        }
       }
       // ---- current-image window of this feature (fine levels): projected with the pose the level starts from
       if constexpr (WIN) {
@@ -1036,6 +1121,8 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       tma_bulk_g2s(stage, cur_img, img_bytes, &s.mbar);
     }
     if (cta_leader) s.st[g & 1u].old_model = s.st[g & 1u].model;  // optimizeGaussNewton: ModelType old_model(model) [EXT]
+    // read by the residual passes, after the barriers of the level setup
+    if (TL && cta_leader) s.cur_tl = reinterpret_cast<const uint4*>(job.cur_tl[level]);
     // next level: pull its current image (coarse levels, staged whole) into L2 while this level iterates
     if (tid == 0 && crank == 0 && level > lvl_lo) {
       const uint32_t nb = ((uint32_t)(P.w[level - 1] * P.h[level - 1]) + 15u) & ~15u;
@@ -1148,6 +1235,9 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
               lo[r] = __funnelshift_r(w0, w1, sh);
               hi[r] = w1 >> sh;
             }
+          } else if constexpr (TL) {
+            // the copy's address is read from shared memory here, not kept in registers across the level
+            fetch5x5_tiled(s.cur_tl, (W + 3) >> 2, ui - 2, vi - 2, lo, hi);
           } else {
 #pragma unroll
             for (int r = 0; r < 5; ++r) fetch8<false>(cur_img, (vi - 2 + r) * W + (ui - 2), lo[r], hi[r]);
@@ -1788,7 +1878,10 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
   for (int b = 0; b < B; ++b) {
     SiaJob& j = jobs[b];
     memset(&j, 0, sizeof(j));
-    for (int l = 0; l < ref[b]->n_levels; ++l) { j.ref_lvl[l] = ref[b]->lvl(l); j.cur_lvl[l] = cur[b]->lvl(l); }
+    for (int l = 0; l < ref[b]->n_levels; ++l) {
+      j.ref_lvl[l] = ref[b]->lvl(l); j.cur_lvl[l] = cur[b]->lvl(l);
+      j.ref_tl[l] = ref[b]->tv[l]; j.cur_tl[l] = cur[b]->tv[l];
+    }
     const int o = feat_offset[b], n = feat_offset[b + 1] - o;
     j.n_feat = n;
     j.n_pad = pad16(n);
