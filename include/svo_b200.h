@@ -212,6 +212,30 @@ typedef struct {
 /* Returns SVO_B200_EINVAL if the context has not launched the alignment kernel yet. */
 int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out);
 
+/* ---- robust cost of SparseImgAlign: vk::NLLSSolver::setRobustCostFunction(scale_estimator, weight_function) ----
+ * Numbering as vikit's ScaleEstimatorType / WeightFunctionType. */
+#define SVO_B200_SCALE_UNIT 0   /* weights off: plain Gauss-Newton, whatever the weight function (default) */
+#define SVO_B200_SCALE_TDIST 1  /* not supported */
+#define SVO_B200_SCALE_MAD 2    /* scale_ = 1.48 * upper median of |res| */
+#define SVO_B200_SCALE_NORMAL 3 /* not supported */
+#define SVO_B200_WEIGHT_UNIT 0
+#define SVO_B200_WEIGHT_TDIST 1 /* not supported */
+#define SVO_B200_WEIGHT_TUKEY 2 /* b = 4.6851 */
+#define SVO_B200_WEIGHT_HUBER 3 /* k = 1.345 */
+/* Context setting like svo_b200_sia_config.  It applies to svo_b200_sparse_img_align and svo_b200_sia_batch_stage (a staged
+ * batch keeps the mode it was staged with); svo_b200_sparse_residuals ignores it.  With weights on (MAD scale) the robust
+ * kernel runs: one CTA per pair, 0..1024 features (SVO_B200_ELIMIT above), every camera model; svo_b200_sia_config and
+ * svo_b200_sia_upfront do not apply to it, and it does not run with a multi-GPU feature split (SVO_B200_EINVAL).
+ * The scale is computed as the reference does it: by the pre-pass each level's Gauss-Newton loop starts with, and only when
+ * iter_ is 0 there -- at the first level, and at a later level only if the previous level's loop ended at iteration 0;
+ * otherwise the scale carries over.  SVO_B200_EINVAL for the T-distribution / normal scales, the T-distribution weight and
+ * values outside the enums. */
+int svo_b200_sia_robust(svo_b200_ctx* ctx, int scale_estimator, int weight_function);
+/* The scale_ each of the B pairs of the last alignment launch used at each level, out[b * SVO_B200_MAX_LEVELS + level]; NaN
+ * outside [min_level, max_level].  Available once the launch's outputs are fetched (svo_b200_sparse_img_align,
+ * svo_b200_sia_batch_fetch).  SVO_B200_EINVAL if the last alignment launch was not weighted or had fewer than B pairs. */
+int svo_b200_sia_last_scales(const svo_b200_ctx* ctx, int B, float* out);
+
 /* ---- one stream's features split over several GPUs (SURVEY.md 8e; a demonstration mode: a pair fits one GPU) ----
  * Every rank (one process or thread per GPU) holds both pyramids and passes ITS contiguous slice of the pair's features
  * to svo_b200_sparse_img_align / svo_b200_sia_batch_*; the kernels of the ranks exchange the per-iteration sums

@@ -40,6 +40,9 @@ class SiaStats(C.Structure):
 
 
 SIA_STAGE_NAMES = {-1: None, 0: "global", 1: "image", 2: "window"}  # SVO_B200_SIA_STAGE_*
+# robust cost (svo_b200_sia_robust): SVO_B200_SCALE_* / SVO_B200_WEIGHT_*, vikit's numbering
+SCALE_UNIT, SCALE_TDIST, SCALE_MAD, SCALE_NORMAL = 0, 1, 2, 3
+WEIGHT_UNIT, WEIGHT_TDIST, WEIGHT_TUKEY, WEIGHT_HUBER = 0, 1, 2, 3
 
 
 class SiaLaunch(C.Structure):
@@ -333,6 +336,18 @@ class Context:
         d = {name: getattr(L, name) for name, _ in SiaLaunch._fields_ if name != "level_stage"}
         d["stages"] = {lv: SIA_STAGE_NAMES[L.level_stage[lv]] for lv in range(L.min_level, L.max_level + 1)}
         return d
+
+    def sia_robust(self, scale=SCALE_UNIT, weight=WEIGHT_UNIT):
+        """Robust cost of the alignment (svo_b200_sia_robust; vk::NLLSSolver::setRobustCostFunction): SCALE_MAD with
+        WEIGHT_UNIT / WEIGHT_TUKEY / WEIGHT_HUBER turns weights on, SCALE_UNIT turns them off."""
+        self._check(self.lib.svo_b200_sia_robust(self.h, int(scale), int(weight)))
+
+    def sia_last_scales(self, B: int = 1) -> np.ndarray:
+        """(B, MAX_LEVELS) float32: the scale each pair's iterations used at each level in the last (weighted) alignment
+        launch, NaN outside [min_level, max_level] (svo_b200_sia_last_scales)."""
+        out = np.zeros((int(B), MAX_LEVELS), np.float32)
+        self._check(self.lib.svo_b200_sia_last_scales(self.h, int(B), _p(out)))
+        return out
 
     def sia_batch_run(self):
         self._check(self.lib.svo_b200_sia_batch_run(self.h))

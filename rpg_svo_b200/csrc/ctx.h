@@ -89,6 +89,10 @@ struct svo_b200_ctx {
   int sia_occ_clusters[2] = {0, 0};
   svo_b200_sia_launch sia_last = {};  // svo_b200_sia_last_launch
   bool sia_last_valid = false;
+  // svo_b200_sia_robust: robust cost of svo_b200_sparse_img_align / svo_b200_sia_batch_stage (UNIT scale = off)
+  int sia_scale_est = SVO_B200_SCALE_UNIT, sia_weight_fn = SVO_B200_WEIGHT_UNIT;
+  bool sia_last_robust = false;   // the last alignment launch ran the robust kernel
+  std::vector<float> sia_scales;  // its per-pair, per-level scales (svo_b200_sia_last_scales), fetched with its outputs
 };
 
 namespace svo {

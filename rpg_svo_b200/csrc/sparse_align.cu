@@ -290,6 +290,47 @@ __device__ __forceinline__ T sel_k(const T (&a)[FPT], int k) {
   return v;
 }
 
+// precomputeReferencePatches' arithmetic (:115-136) for one feature: the 4x4 reference patch and its two gradient images
+// from the 7x7 footprint (rows vi-3..vi+3, columns ui-3..ui+3; row r = bytes 0..3 of lo[r], 0..2 of hi[r]) at the sub-pixel
+// offset (su, sv).  The footprint is streamed row by row to keep the register footprint small: Bq row r (bilinear blends
+// with top-left tap P[r][c]) needs footprint rows r, r+1; patch row y needs Bq rows y, y+1, y+2.  emit(p, val, dx, dy) takes
+// pixel p = 4 y + x.  The same operations in the same order as level_patches in sia_kernel, which keeps them inline: called
+// from there, this function changes the local-memory slot assignment of ten of its instantiations.
+template <class Emit>
+__device__ __forceinline__ void ref_patch_7x7(const uint32_t (&rlo)[7], const uint32_t (&rhi)[7], float su, float sv, Emit emit) {
+  float wtl, wtr, wbl, wbr;
+  bilin_weights(su, sv, wtl, wtr, wbl, wbr);
+  float pr0[7], pr1[7], b0[6], b1[6], b2[6];
+  auto load_row = [&](int r, float (&dst)[7]) {
+    const uint32_t lo = rlo[r], hi = rhi[r];
+    dst[0] = byte_to_float<0>(lo); dst[1] = byte_to_float<1>(lo); dst[2] = byte_to_float<2>(lo);
+    dst[3] = byte_to_float<3>(lo); dst[4] = byte_to_float<0>(hi); dst[5] = byte_to_float<1>(hi);
+    dst[6] = byte_to_float<2>(hi);
+  };
+  load_row(0, pr0);
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+    load_row(r + 1, pr1);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) b2[c] = bilin(wtl, wtr, wbl, wbr, pr0[c], pr0[c + 1], pr1[c], pr1[c + 1]);
+    if (r >= 2) {  // rows b0 (= Bq[y]), b1 (= Bq[y+1]), b2 (= Bq[y+2]) with y = r-2 are complete
+      const int y = r - 2;
+#pragma unroll
+      for (int x = 0; x < 4; ++x) {
+        const int p = y * 4 + x;
+        const float val = b1[x + 1];
+        const float dx = __fmul_rn(0.5f, __fsub_rn(b1[x + 2], b1[x]));
+        const float dy = __fmul_rn(0.5f, __fsub_rn(b2[x + 1], b0[x + 1]));
+        emit(p, val, dx, dy);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 6; ++c) { b0[c] = b1[c]; b1[c] = b2[c]; }
+#pragma unroll
+    for (int c = 0; c < 7; ++c) pr0[c] = pr1[c];
+  }
+}
+
 // per-feature unscaled Jacobian rows: a = row0 of jacobian_xyz2uv, b = row1 (frame.h:116-138)
 __device__ __forceinline__ void jac_rows(double x, double y, double zi, double (&a)[6], double (&b)[6]) {
   const double X = x * zi, Y = y * zi;
@@ -1491,6 +1532,365 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
 }
 
 // =============================================================================================
+// Robust cost (NLLSSolver::setRobustCostFunction with MADScale; DESIGN.md 4.1c)
+// =============================================================================================
+// With a per-pixel weight H is no longer pose independent, so the factorisation of sia_kernel (H summed and factorised once
+// per level) does not apply: this kernel re-sums the weighted H from per-feature weighted moments and factorises it in every
+// iteration.  One CTA per pair, kSiaRobustThreads threads, features dealt round robin (feature i to thread i % T); the
+// reference patches, gradients and xyz_ref of all the pair's features live in shared memory, the current image is read from
+// global memory.  It is a kernel of its own so that the instantiations of sia_kernel keep their code.
+constexpr int kSiaRobustThreads = 256;
+constexpr int kSiaRobustWarps = kSiaRobustThreads / 32;
+constexpr int kSiaRobustMaxFeat = 1024;
+
+struct SiaRobustParams {
+  SiaParams P;        // jobs, pyramid, camera, levels, iterations and the outputs of sia_kernel (EVAL fields unused)
+  int weight;         // SVO_B200_WEIGHT_UNIT / _TUKEY / _HUBER
+  int slots;          // stride of the per-feature shared arrays (>= the largest feature count of the batch)
+  float* scales_out;  // [B][SVO_B200_MAX_LEVELS]: scale_ the iterations of each level used, NaN outside [min, max]
+};
+
+struct SiaRobustShared {
+  SiaState st[2];                       // double-buffered by the running iteration counter, as in sia_kernel
+  double part[kSiaRobustWarps][32];     // per-warp sums: 21 H entries, 6 Jres, chi2 (slots 28..31 unused)
+  double sums[kPartK];                  // pair totals of the 21 H entries (warp_scale_and_factor reads them)
+  double Hs[36];                        // H_ of the last pass (scaled, full symmetric)
+  Solver6 sol;
+  alignas(16) double pub[12];           // the pose warp 0 publishes after its Gauss-Newton tail
+  unsigned hist[256];                   // radix-select histogram
+  int cnt[kSiaRobustWarps];
+  int n_in_last, n_iters, sum_vis, sum_in, n_trace;  // gn_tail's counters (thread 0)
+  int pub_done, sel_bin, sel_k, n_pre;
+#if SVO_SIA_DEBUG
+  long long tk[8];
+#endif
+};
+__host__ __device__ constexpr size_t sia_robust_ctl_bytes() { return (sizeof(SiaRobustShared) + 15) & ~size_t(15); }
+// dynamic shared memory: control block, [16][SA] f32 reference patch, [16][SA] float2 gradients, [3][SA] f64 xyz_ref
+__host__ __device__ constexpr size_t sia_robust_smem_bytes(int slots) {
+  return sia_robust_ctl_bytes() + (size_t)slots * (kPatchArea * (sizeof(float) + sizeof(float2)) + 3 * sizeof(double));
+}
+
+// [EXT] vk::robust_cost weight functions restated in f32 (oracle/svo_oracle_robust.cpp): x = res / scale_.
+__device__ __forceinline__ float robust_weight(int wf, float res, float scale) {
+  const float x = __fdiv_rn(res, scale);
+  if (wf == SVO_B200_WEIGHT_TUKEY) {  // b = 4.6851
+    constexpr float b2 = 4.6851f * 4.6851f;
+    const float x2 = __fmul_rn(x, x);
+    if (x2 <= b2) {
+      const float tmp = __fsub_rn(1.0f, __fdiv_rn(x2, b2));
+      return __fmul_rn(tmp, tmp);
+    }
+    return 0.0f;  // also for x = +-inf and NaN
+  }
+  if (wf == SVO_B200_WEIGHT_HUBER) {  // k = 1.345: NaN for x = NaN (0 / 0)
+    const float t = fabsf(x);
+    return t < 1.345f ? 1.0f : __fdiv_rn(1.345f, t);
+  }
+  return 1.0f;
+}
+
+__global__ void __launch_bounds__(kSiaRobustThreads, 1) sia_robust_kernel(const SiaRobustParams RP) {
+  const SiaParams& P = RP.P;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SiaRobustShared& s = *reinterpret_cast<SiaRobustShared*>(smem_raw);
+  const int SA = RP.slots;
+  float* const pat_ref = reinterpret_cast<float*>(smem_raw + sia_robust_ctl_bytes());  // [16][SA]
+  float2* const pat_dxy = reinterpret_cast<float2*>(pat_ref + kPatchArea * SA);        // [16][SA]
+  double* const xyz = reinterpret_cast<double*>(pat_dxy + kPatchArea * SA);            // [3][SA]
+  constexpr int T = kSiaRobustThreads, FPT = kSiaRobustMaxFeat / kSiaRobustThreads;
+  const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const SiaJob& job = P.jobs[pair];
+  const int N = job.n_feat, np = job.n_pad;
+  const bool leader = tid == 0;
+  const double* b_px = reinterpret_cast<const double*>(job.blob);
+  const double* b_f = b_px + 2 * np;
+  const double* b_pos = b_f + 3 * np;
+  const uint8_t* b_hp = reinterpret_cast<const uint8_t*>(b_pos + 3 * np);
+
+  // xyz_ref = f * |pos - ref_pos| (:107-108), as sia_kernel forms it
+  for (int i = tid; i < N; i += T) {
+    const double dxp = b_pos[3 * i] - job.ref_pos[0], dyp = b_pos[3 * i + 1] - job.ref_pos[1], dzp = b_pos[3 * i + 2] - job.ref_pos[2];
+    const double depth = sqrt(dxp * dxp + dyp * dyp + dzp * dzp);
+    xyz[i] = b_f[3 * i] * depth;
+    xyz[SA + i] = b_f[3 * i + 1] * depth;
+    xyz[2 * SA + i] = b_f[3 * i + 2] * depth;
+  }
+  double R[9], t[3];
+  if (leader) {
+    s.st[0].model = pose_from_rt12(job.T);
+    s.st[0].old_model = s.st[0].model;
+    s.n_in_last = 0; s.n_iters = 0; s.sum_vis = 0; s.sum_in = 0; s.n_trace = 0;
+    for (int k = 0; k < 36; ++k) s.Hs[k] = 0.0;
+    qmatrix(s.st[0].model.q, R);
+    for (int k = 0; k < 9; ++k) s.pub[k] = R[k];
+    for (int k = 0; k < 3; ++k) s.pub[9 + k] = s.st[0].model.t[k];
+    if (RP.scales_out)
+      for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) RP.scales_out[(size_t)pair * SVO_B200_MAX_LEVELS + l] = __int_as_float(0x7fc00000);
+  }
+  __syncthreads();
+  auto load_pose = [&]() {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) R[k] = s.pub[k];
+    t[0] = s.pub[9]; t[1] = s.pub[10]; t[2] = s.pub[11];
+  };
+  load_pose();
+
+  // The feature's 16 residuals at the current pose (computeResiduals :179-210): false if the patch is outside the current
+  // image (:190).  emit(p, res, gradient) per pixel.
+  auto residuals = [&](int i, int W, int Hh, float scale, const uint8_t* cur_img, auto emit) -> bool {
+    const double x = xyz[i], y = xyz[SA + i], z = xyz[2 * SA + i];
+    const double xc = fma(R[0], x, fma(R[1], y, fma(R[2], z, t[0])));
+    const double yc = fma(R[3], x, fma(R[4], y, fma(R[5], z, t[1])));
+    const double zc = fma(R[6], x, fma(R[7], y, fma(R[8], z, t[2])));
+    const double rz = fast_rcp(zc);
+    double ud, vd;
+    cam_world2cam(P.cam, div_rn(xc, zc, rz), div_rn(yc, zc, rz), ud, vd);
+    const float u_cur = __fmul_rn((float)ud, scale), v_cur = __fmul_rn((float)vd, scale);
+    const bool rng = u_cur >= 0.f && v_cur >= 0.f && u_cur < 1e6f && v_cur < 1e6f;
+    float ufl = 0.f, vfl = 0.f;
+    const int ui = rng ? floor_pos(u_cur, ufl) : -1, vi = rng ? floor_pos(v_cur, vfl) : -1;
+    if (!(ui - 3 >= 0 && vi - 3 >= 0 && ui + 3 < W && vi + 3 < Hh)) return false;
+    float wtl, wtr, wbl, wbr;
+    bilin_weights(__fsub_rn(u_cur, ufl), __fsub_rn(v_cur, vfl), wtl, wtr, wbl, wbr);
+    uint32_t lo[5], hi[5];
+#pragma unroll
+    for (int r = 0; r < 5; ++r) fetch8<false>(cur_img, (vi - 2 + r) * W + (ui - 2), lo[r], hi[r]);
+    float q0[5], q1[5];
+    q0[0] = byte_to_float<0>(lo[0]); q0[1] = byte_to_float<1>(lo[0]); q0[2] = byte_to_float<2>(lo[0]);
+    q0[3] = byte_to_float<3>(lo[0]); q0[4] = byte_to_float<0>(hi[0]);
+#pragma unroll
+    for (int yy = 0; yy < 4; ++yy) {
+      q1[0] = byte_to_float<0>(lo[yy + 1]); q1[1] = byte_to_float<1>(lo[yy + 1]); q1[2] = byte_to_float<2>(lo[yy + 1]);
+      q1[3] = byte_to_float<3>(lo[yy + 1]); q1[4] = byte_to_float<0>(hi[yy + 1]);
+#pragma unroll
+      for (int xx = 0; xx < 4; ++xx) {
+        const int p = yy * 4 + xx;
+        const float I = bilin(wtl, wtr, wbl, wbr, q0[xx], q0[xx + 1], q1[xx], q1[xx + 1]);
+        emit(p, __fsub_rn(I, pat_ref[p * SA + i]), pat_dxy[p * SA + i]);
+      }
+#pragma unroll
+      for (int c = 0; c < 5; ++c) q0[c] = q1[c];
+    }
+    return true;
+  };
+
+  double chi2_prev = 1e10;  // chi2_ of NLLSSolver::reset() [EXT]
+  int stop = 0;
+  unsigned g = 0;
+  float wscale = 0.0f;   // scale_ (NLLSSolver() initialises it to 0 [EXT])
+  int iter_end = 0;      // iter_ as the previous level's loop left it (reset(): 0)
+  long long n_meas_pre = 0;  // n_meas_ counted by the pre-calls (reset only by the loop)
+  unsigned vis_mask = 0;     // bit k: feature tid + k T is visible (set-only across levels, :57)
+  for (int level = P.max_level; level >= P.min_level; --level) {
+    const int W = P.w[level], Hh = P.h[level];
+    const float scale = 1.0f / (float)(1 << level);
+    const double jscale = P.cam.fx / (double)(1 << level);
+    const uint8_t* ref_img = job.ref_lvl[level];
+    const uint8_t* cur_img = job.cur_lvl[level];
+    // ---- precomputeReferencePatches (:84-145)
+    int n_vis_t = 0;
+#pragma unroll 1
+    for (int k = 0; k < FPT; ++k) {
+      const int i = tid + k * T;
+      if (i >= N) break;
+      const float u_ref = (float)(b_px[2 * i] * (double)scale), v_ref = (float)(b_px[2 * i + 1] * (double)scale);
+      const bool rng = u_ref >= 0.f && v_ref >= 0.f && u_ref < 1e6f && v_ref < 1e6f;
+      float ufl = 0.f, vfl = 0.f;
+      const int ui = rng ? floor_pos(u_ref, ufl) : -1, vi = rng ? floor_pos(v_ref, vfl) : -1;
+      if (b_hp[i] && ui - 3 >= 0 && vi - 3 >= 0 && ui + 3 < W && vi + 3 < Hh) {
+        vis_mask |= 1u << k;
+        uint32_t rlo[7], rhi[7];
+#pragma unroll
+        for (int r = 0; r < 7; ++r) fetch7_g64(ref_img, (vi - 3 + r) * W + (ui - 3), rlo[r], rhi[r]);
+        ref_patch_7x7(rlo, rhi, __fsub_rn(u_ref, ufl), __fsub_rn(v_ref, vfl), [&](int p, float val, float dx, float dy) {
+          pat_ref[p * SA + i] = val;
+          pat_dxy[p * SA + i] = make_float2(dx, dy);
+        });
+      } else if ((vis_mask >> k) & 1u) {  // visible at a coarser level only: stale patch, zero Jacobian (as sia_kernel)
+        for (int p = 0; p < kPatchArea; ++p) pat_dxy[p * SA + i] = make_float2(0.f, 0.f);
+      }
+      n_vis_t += (vis_mask >> k) & 1u;
+    }
+    n_vis_t = __reduce_add_sync(0xffffffffu, n_vis_t);
+    if (lane == 0) s.cnt[warp] = n_vis_t;
+    if (leader) s.st[g & 1u].old_model = s.st[g & 1u].model;
+    __syncthreads();
+    if (leader) for (int w = 0; w < kSiaRobustWarps; ++w) s.sum_vis += s.cnt[w];
+
+    // ---- the pre-call computeResiduals(model, false, true) of optimizeGaussNewton [EXT]: counts n_meas_ and, when iter_ is
+    //      0 (:239), sets scale_ = 1.48 * the upper median of |res| (MAD) -- an exact MSB-first radix select on the bit
+    //      patterns of the non-negative f32 |res| (ordered like the values), 8 bits per sweep; every sweep recomputes the
+    //      residuals instead of storing 16 N of them.
+    {
+      const bool want_scale = iter_end == 0;
+      unsigned prefix = 0, pmask = 0;
+      int kth = 0;
+      for (int sweep = 0; sweep < (want_scale ? 4 : 1); ++sweep) {
+        const int shift = 24 - 8 * sweep;
+        for (int b = tid; b < 256; b += T) s.hist[b] = 0u;
+        __syncthreads();
+        int n_in_t = 0;
+#pragma unroll 1
+        for (int k = 0; k < FPT; ++k) {
+          const int i = tid + k * T;
+          if (i >= N) break;
+          if (!((vis_mask >> k) & 1u)) continue;
+          n_in_t += residuals(i, W, Hh, scale, cur_img, [&](int, float res, float2) {
+            const unsigned key = __float_as_uint(fabsf(res));
+            if (want_scale && (key & pmask) == prefix) atomicAdd(&s.hist[(key >> shift) & 255u], 1u);
+          });
+        }
+        if (sweep == 0) {
+          n_in_t = __reduce_add_sync(0xffffffffu, n_in_t);
+          if (lane == 0) s.cnt[warp] = n_in_t;
+        }
+        __syncthreads();
+        if (sweep == 0) {
+          int n = 0;
+          for (int w = 0; w < kSiaRobustWarps; ++w) n += s.cnt[w];
+          if (leader) s.n_pre = n;
+          n_meas_pre += (long long)n * kPatchArea;
+          // getMedian of no errors is undefined in the reference: scale_ stays (not pinned)
+          if (n == 0 || !want_scale) break;
+          kth = n * kPatchArea / 2;  // vk::getMedian: nth_element at floor(n / 2)
+        }
+        if (warp == 0) {  // lane l scans bins [8 l, 8 l + 8)
+          unsigned loc[8], sum = 0;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) { loc[j] = s.hist[8 * lane + j]; sum += loc[j]; }
+          unsigned inc = sum;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const unsigned v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+          }
+          const unsigned hit = __ballot_sync(0xffffffffu, inc > (unsigned)kth);
+          if (lane == __ffs(hit) - 1) {
+            unsigned cum = inc - sum;
+            int bin = 8 * lane;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              if (cum + loc[j] > (unsigned)kth) { bin = 8 * lane + j; break; }
+              cum += loc[j];
+            }
+            s.sel_bin = bin;
+            s.sel_k = kth - (int)cum;
+          }
+        }
+        __syncthreads();
+        prefix |= (unsigned)s.sel_bin << shift;
+        pmask |= 255u << shift;
+        kth = s.sel_k;
+        if (sweep == 3) wscale = __fmul_rn(1.48f, __uint_as_float(prefix));  // MADScaleEstimator [EXT]
+        __syncthreads();  // s.sel_* and s.hist are rewritten by the next sweep
+      }
+    }
+    if (leader && RP.scales_out) RP.scales_out[(size_t)pair * SVO_B200_MAX_LEVELS + level] = wscale;
+
+    // ---- Gauss-Newton iterations: every pass re-sums the weighted H and factorises it
+    iter_end = P.n_iter;
+    for (int iter = 0; iter < P.n_iter; ++iter) {
+      double acc[32];
+#pragma unroll
+      for (int e = 0; e < 32; ++e) acc[e] = 0.0;
+      int n_in_t = 0;
+#pragma unroll 1
+      for (int k = 0; k < FPT; ++k) {
+        const int i = tid + k * T;
+        if (i >= N) break;
+        if (!((vis_mask >> k) & 1u)) continue;
+        // weighted moments of the patch: sum w dx^2, w dx dy, w dy^2, w dx r, w dy r (f64) and chi2 += res^2 w (f32, :222)
+        double sxx = 0.0, sxy = 0.0, syy = 0.0, sxr = 0.0, syr = 0.0;
+        float c2 = 0.f;
+        const bool in = residuals(i, W, Hh, scale, cur_img, [&](int, float res, float2 gr) {
+          const float w = robust_weight(RP.weight, res, wscale);
+          c2 = fmaf(__fmul_rn(res, res), w, c2);
+          const double wd = (double)w, dx = (double)gr.x, dy = (double)gr.y, r = (double)res;
+          sxx = fma(wd * dx, dx, sxx);
+          sxy = fma(wd * dx, dy, sxy);
+          syy = fma(wd * dy, dy, syy);
+          sxr = fma(wd * dx, r, sxr);
+          syr = fma(wd * dy, r, syr);
+        });
+        if (!in) continue;
+        ++n_in_t;
+        const double z = xyz[2 * SA + i];
+        double a[6], b[6];
+        jac_rows(xyz[i], xyz[SA + i], rcp_rn(z), a, b);
+#define SIA_ROBUST_H(IDX) acc[IDX] += h_entry<IDX>(a, b, sxx, sxy, syy);
+        SIA_ROBUST_H(0) SIA_ROBUST_H(1) SIA_ROBUST_H(2) SIA_ROBUST_H(3) SIA_ROBUST_H(4) SIA_ROBUST_H(5) SIA_ROBUST_H(6)
+        SIA_ROBUST_H(7) SIA_ROBUST_H(8) SIA_ROBUST_H(9) SIA_ROBUST_H(10) SIA_ROBUST_H(11) SIA_ROBUST_H(12) SIA_ROBUST_H(13)
+        SIA_ROBUST_H(14) SIA_ROBUST_H(15) SIA_ROBUST_H(16) SIA_ROBUST_H(17) SIA_ROBUST_H(18) SIA_ROBUST_H(19) SIA_ROBUST_H(20)
+#undef SIA_ROBUST_H
+#pragma unroll
+        for (int e = 0; e < 6; ++e) acc[21 + e] = fma(a[e], sxr, fma(b[e], syr, acc[21 + e]));
+        acc[27] += (double)c2;
+      }
+      // ---- pair sums: four transposed 8-value warp reductions, one shared-memory hop, warp 0 adds the warps' partials
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        double v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = acc[8 * c + j];
+        warp_reduce_t<8>(v);
+        if ((lane & 3) == 0) s.part[warp][8 * c + (lane >> 2)] = v[0];
+      }
+      n_in_t = __reduce_add_sync(0xffffffffu, n_in_t);
+      if (lane == 0) s.cnt[warp] = n_in_t;
+      __syncthreads();
+      if (warp == 0) {
+        double tot_l = 0.0;
+        int n_in = 0;
+        for (int w = 0; w < kSiaRobustWarps; ++w) { tot_l += s.part[w][lane]; n_in += s.cnt[w]; }
+        if (lane < 21) s.sums[lane] = tot_l;
+        double tot[7];
+#pragma unroll
+        for (int e = 0; e < 7; ++e) tot[e] = __shfl_sync(0xffffffffu, tot_l, 21 + e);
+        __syncwarp();
+        warp_scale_and_factor(s.sums, jscale * jscale, s.Hs, s.sol);
+        int done = 0;
+        gn_tail(s, g, &s.sol, tot, jscale, n_in, iter, level, P.eps, leader, leader, P.trace, P.trace_cap, chi2_prev, stop, done,
+                R, t);
+        if (lane == 0) {
+#pragma unroll
+          for (int k = 0; k < 9; ++k) s.pub[k] = R[k];
+          s.pub[9] = t[0]; s.pub[10] = t[1]; s.pub[11] = t[2];
+          s.pub_done = done;
+        }
+      }
+      __syncthreads();
+      load_pose();
+      const int done = s.pub_done;  // (chi2_ and stop_ live in warp 0, which alone runs the tail)
+      ++g;
+      __syncthreads();  // s.pub_done / s.part are rewritten by the next pass
+      if (done) { iter_end = iter; break; }
+    }
+  }
+
+  // ---- outputs
+#pragma unroll 1
+  for (int k = 0; k < FPT; ++k) {
+    const int i = tid + k * T;
+    if (i < N && P.visible_out) P.visible_out[job.feat_off + i] = (vis_mask >> k) & 1u;
+  }
+  if (leader) {
+    if (P.T_out) pose_to_rt12(s.st[g & 1u].model, P.T_out + 12 * (size_t)pair);
+    if (P.H_out)
+      for (int k = 0; k < 36; ++k) P.H_out[36 * (size_t)pair + k] = s.Hs[k];
+    if (P.stats) {
+      svo_b200_sia_stats st;
+      st.n_iters = s.n_iters; st.sum_visible = s.sum_vis; st.sum_in_image = s.sum_in;
+      // run() returns n_meas_ / patch_area_ (:74): the last pass's count, or -- no iteration ran at all -- what the pre-calls
+      // of every level added up (only the loop resets n_meas_)
+      st.n_tracked = P.n_iter > 0 ? s.n_in_last : (int)(n_meas_pre / kPatchArea);
+      P.stats[pair] = st;
+    }
+    if (P.n_trace) *P.n_trace = s.n_trace;
+  }
+}
+
+// =============================================================================================
 // Host side
 // =============================================================================================
 using SiaKernel = void (*)(SiaParams);
@@ -1548,9 +1948,13 @@ struct SiaBatchState {
   DevBuf d_in, d_out;
   HostBuf h_in, h_out;
   size_t o_T = 0, o_H = 0, o_vis = 0, o_stats = 0, out_bytes = 0;
-  const SiaEntry* geo = nullptr;  // the launch geometry pick_launch chose
+  const SiaEntry* geo = nullptr;  // the launch geometry pick_launch chose (nullptr: the robust kernel)
   size_t smem = 0;
   bool staged = false;
+  // robust cost (svo_b200_sia_robust) the batch was staged with: weight function, or -1 = unweighted (sia_kernel)
+  int robust_weight = -1;
+  int robust_slots = 0;
+  size_t o_scales = 0;
 };
 
 void sia_batch_free(svo_b200_ctx* ctx) {
@@ -1713,6 +2117,35 @@ static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, const SiaEnt
   for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l)
     L.level_stage[l] = l >= L.min_level && l <= L.max_level ? sia_stage_mode(sia_image_bytes(P.w[l], P.h[l]), P.w[l], P.stage_cap, e->windows, e->slots) : -1;
   ctx->sia_last_valid = true;
+  ctx->sia_last_robust = false;
+  return 0;
+}
+
+// Launches the robust kernel for a staged batch and records it for svo_b200_sia_last_launch / svo_b200_sia_last_scales.
+static int launch_sia_robust(svo_b200_ctx* ctx, const SiaBatchState& st) {
+  SiaRobustParams RP;
+  RP.P = st.P;
+  RP.weight = st.robust_weight;
+  RP.slots = st.robust_slots;
+  RP.scales_out = reinterpret_cast<float*>(static_cast<uint8_t*>(st.d_out.p) + st.o_scales);
+  SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(sia_robust_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.smem));
+  kt_begin(ctx);
+  sia_robust_kernel<<<st.B, kSiaRobustThreads, st.smem, ctx->stream>>>(RP);
+  kt_end(ctx);
+  ctx->launches++;
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  svo_b200_sia_launch& L = ctx->sia_last;
+  L = svo_b200_sia_launch{};
+  L.n_pairs = st.B; L.ctas_per_pair = 1; L.threads = kSiaRobustThreads;
+  L.features_per_thread = (st.max_feat + kSiaRobustThreads - 1) / kSiaRobustThreads;
+  L.min_blocks = 1; L.upfront = 0; L.general_camera = 1; L.residuals_only = 0; L.stage_cap = 0; L.smem_bytes = (int)st.smem;
+  L.resident_clusters = ctx->sia_occ_clusters[0];
+  L.sm_count = ctx->sm_count;
+  L.min_level = st.P.min_level; L.max_level = st.P.max_level;
+  for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) L.level_stage[l] = l >= L.min_level && l <= L.max_level ? SVO_B200_SIA_STAGE_GLOBAL : -1;
+  ctx->sia_last_valid = true;
+  ctx->sia_last_robust = true;
+  ctx->sia_scales.assign((size_t)st.B * SVO_B200_MAX_LEVELS, __builtin_nanf(""));  // filled by svo_b200_sia_batch_fetch
   return 0;
 }
 
@@ -1822,6 +2255,39 @@ int svo_b200_sia_upfront(svo_b200_ctx* ctx, int mode) {
   return 0;
 }
 
+int svo_b200_sia_robust(svo_b200_ctx* ctx, int scale_estimator, int weight_function) {
+  if (!ctx) return SVO_B200_EINVAL;
+  if (scale_estimator < SVO_B200_SCALE_UNIT || scale_estimator > SVO_B200_SCALE_NORMAL || weight_function < SVO_B200_WEIGHT_UNIT ||
+      weight_function > SVO_B200_WEIGHT_HUBER)
+    return set_err(ctx, SVO_B200_EINVAL, "sia_robust: scale estimator %d / weight function %d is not an SVO_B200_SCALE_* / SVO_B200_WEIGHT_* value",
+                   scale_estimator, weight_function);
+  if (scale_estimator == SVO_B200_SCALE_UNIT) {  // use_weights_ = false: plain Gauss-Newton whatever the weight function
+    ctx->sia_scale_est = SVO_B200_SCALE_UNIT;
+    ctx->sia_weight_fn = SVO_B200_WEIGHT_UNIT;
+    return 0;
+  }
+  if (scale_estimator != SVO_B200_SCALE_MAD)
+    return set_err(ctx, SVO_B200_EINVAL, "sia_robust: only the MAD scale estimator is supported (T-distribution and normal scales are not)");
+  if (weight_function == SVO_B200_WEIGHT_TDIST)
+    return set_err(ctx, SVO_B200_EINVAL, "sia_robust: the T-distribution weight function is not supported (unit, Tukey or Huber)");
+  if (ctx->xg_connected)
+    return set_err(ctx, SVO_B200_EINVAL, "sia_robust: the robust cost does not run with a multi-GPU feature split");
+  ctx->sia_scale_est = scale_estimator;
+  ctx->sia_weight_fn = weight_function;
+  return 0;
+}
+
+int svo_b200_sia_last_scales(const svo_b200_ctx* ctx, int B, float* out) {
+  if (!ctx || !out || B < 1) return SVO_B200_EINVAL;
+  if (!ctx->sia_last_valid || !ctx->sia_last_robust)
+    return set_err(const_cast<svo_b200_ctx*>(ctx), SVO_B200_EINVAL, "sia_last_scales: the last alignment launch was not weighted");
+  if ((size_t)B * SVO_B200_MAX_LEVELS > ctx->sia_scales.size())
+    return set_err(const_cast<svo_b200_ctx*>(ctx), SVO_B200_EINVAL, "sia_last_scales: the last launch had %d pairs",
+                   (int)(ctx->sia_scales.size() / SVO_B200_MAX_LEVELS));
+  memcpy(out, ctx->sia_scales.data(), sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)B);
+  return 0;
+}
+
 int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out) {
   if (!ctx || !out) return SVO_B200_EINVAL;
   if (!ctx->sia_last_valid) return set_err(const_cast<svo_b200_ctx*>(ctx), SVO_B200_EINVAL, "sia_last_launch: no alignment kernel launched yet");
@@ -1829,11 +2295,14 @@ int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out) 
   return 0;
 }
 
-int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
-                             const svo_b200_frame* const* cur, const svo_b200_camera* cam,
-                             const svo_b200_sia_options* opt, const double* T, const int* feat_offset,
-                             const double* px, const double* f, const double* point_pos,
-                             const uint8_t* has_point, const double* ref_pos) {
+}  // extern "C"
+
+namespace svo {
+// svo_b200_sia_batch_stage with the robust cost of the context (`robust`) or without it (svo_b200_sparse_residuals).
+static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref, const svo_b200_frame* const* cur,
+                     const svo_b200_camera* cam, const svo_b200_sia_options* opt, const double* T, const int* feat_offset,
+                     const double* px, const double* f, const double* point_pos, const uint8_t* has_point, const double* ref_pos,
+                     bool robust) {
   if (!ctx || B <= 0 || !ref || !cur || !cam || !opt || !T || !feat_offset || !ref_pos)
     return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: bad arguments");
   cudaSetDevice(ctx->device);
@@ -1856,8 +2325,24 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
     return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: NULL feature arrays");
   int rc = fill_common(ctx, st.P, ref[0], cam, opt);
   if (rc) return rc;
-  rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.geo, st.P.stage_cap, st.smem);
-  if (rc) return rc;
+  // weights on: the robust kernel, chosen before pick_launch (svo_b200_sia_config / _upfront do not apply to it)
+  const bool weighted = robust && ctx->sia_scale_est == SVO_B200_SCALE_MAD;
+  st.robust_weight = -1;
+  if (weighted) {
+    if (ctx->xg_connected)
+      return set_err(ctx, SVO_B200_EINVAL, "sparse_img_align: the robust cost does not run with a multi-GPU feature split");
+    if (st.max_feat > kSiaRobustMaxFeat)
+      return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features per pair > %d (robust cost)", st.max_feat, kSiaRobustMaxFeat);
+    st.robust_slots = ((st.max_feat > 1 ? st.max_feat : 1) + 31) & ~31;
+    st.smem = sia_robust_smem_bytes(st.robust_slots);
+    if (st.smem > (size_t)ctx->max_smem_optin)
+      return set_err(ctx, SVO_B200_ELIMIT, "sparse_img_align: %d features need %zu B of shared memory (robust cost)", st.max_feat, st.smem);
+    st.geo = nullptr;
+    st.robust_weight = ctx->sia_weight_fn;
+  } else {
+    rc = pick_launch(ctx, B, st.max_feat, opt->max_level - opt->min_level + 1, st.geo, st.P.stage_cap, st.smem);
+    if (rc) return rc;
+  }
 
   // input staging: [jobs B][blobs]
   Carver cin;
@@ -1899,6 +2384,7 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
   st.o_H = co.take(sizeof(double) * 36 * (size_t)B);
   st.o_stats = co.take(sizeof(svo_b200_sia_stats) * (size_t)B);
   st.o_vis = co.take((size_t)st.total_feat + 16);
+  if (weighted) st.o_scales = co.take(sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)B);
   st.out_bytes = co.off;
   if ((rc = ensure_dev(ctx, st.d_out, st.out_bytes))) return rc;
   if ((rc = ensure_host(ctx, st.h_out, st.out_bytes))) return rc;
@@ -1911,11 +2397,23 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
   st.staged = true;
   return 0;
 }
+}  // namespace svo
+
+extern "C" {
+
+int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
+                             const svo_b200_frame* const* cur, const svo_b200_camera* cam,
+                             const svo_b200_sia_options* opt, const double* T, const int* feat_offset,
+                             const double* px, const double* f, const double* point_pos,
+                             const uint8_t* has_point, const double* ref_pos) {
+  return sia_stage(ctx, B, ref, cur, cam, opt, T, feat_offset, px, f, point_pos, has_point, ref_pos, true);
+}
 
 int svo_b200_sia_batch_run(svo_b200_ctx* ctx) {
   if (!ctx || !ctx->sia || !ctx->sia->staged) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_run: nothing staged");
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
+  if (st.robust_weight >= 0) return launch_sia_robust(ctx, st);
   return launch_sia(ctx, st.P, st.B, *st.geo, st.smem, false);
 }
 
@@ -1938,6 +2436,8 @@ int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_
   if (H_out) memcpy(H_out, h + st.o_H, sizeof(double) * 36 * (size_t)st.B);
   if (stats_out) memcpy(stats_out, h + st.o_stats, sizeof(svo_b200_sia_stats) * (size_t)st.B);
   if (visible_out) memcpy(visible_out, h + st.o_vis, (size_t)st.total_feat);
+  if (st.robust_weight >= 0 && ctx->sia_last_robust && ctx->sia_scales.size() == (size_t)st.B * SVO_B200_MAX_LEVELS)
+    memcpy(ctx->sia_scales.data(), h + st.o_scales, sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)st.B);
   return 0;
 }
 
@@ -1999,7 +2499,7 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
     return set_err(ctx, SVO_B200_EINVAL, "sparse_residuals: bad arguments");
   svo_b200_sia_options opt = {level, level, 1, 1e-6};
   const int off[2] = {0, N};
-  int rc = svo_b200_sia_batch_stage(ctx, 1, &ref, &cur, cam, &opt, T, off, px, f, point_pos, has_point, ref_pos);
+  int rc = sia_stage(ctx, 1, &ref, &cur, cam, &opt, T, off, px, f, point_pos, has_point, ref_pos, false);  // never weighted
   if (rc) return rc;
   SiaBatchState& st = *ctx->sia;
   const size_t nslots = (size_t)st.geo->threads * st.geo->fpt * st.geo->cluster;

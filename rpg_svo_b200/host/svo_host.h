@@ -303,10 +303,23 @@ inline bool Point::getCloseViewObs(const Vector3d& framepos, Feature*& ftr) cons
 class SparseImgAlign {
  public:
   enum Method { GaussNewton, LevenbergMarquardt };  // [EXT] vk::NLLSSolver::Method; only GaussNewton is used
+  // [EXT] vk::NLLSSolver's robust cost, vikit's numbering (= SVO_B200_SCALE_* / SVO_B200_WEIGHT_*)
+  enum ScaleEstimatorType { UnitScale, TDistScale, MADScale, NormalScale };
+  enum WeightFunctionType { UnitWeight, TDistWeight, TukeyWeight, HuberWeight };
   SparseImgAlign(int max_level, int min_level, int n_iter, Method method, bool /*display*/, bool /*verbose*/)
       : max_level_(max_level), min_level_(min_level), n_iter_(n_iter) {
     if (method != GaussNewton) throw std::invalid_argument("SparseImgAlign: only GaussNewton is implemented");
     H_.fill(0.0);
+  }
+  // [EXT] NLLSSolver::setRobustCostFunction: every scale estimator but UnitScale turns weights on (UnitScale: plain
+  // Gauss-Newton whatever the weight function).  Supported: MADScale with UnitWeight, TukeyWeight or HuberWeight.
+  void setRobustCostFunction(ScaleEstimatorType scale_estimator, WeightFunctionType weight_function) {
+    if (scale_estimator == TDistScale || scale_estimator == NormalScale)
+      throw std::invalid_argument("SparseImgAlign::setRobustCostFunction: only the MAD and unit scale estimators are implemented");
+    if (scale_estimator == MADScale && weight_function == TDistWeight)
+      throw std::invalid_argument("SparseImgAlign::setRobustCostFunction: the T-distribution weight is not implemented");
+    scale_estimator_ = scale_estimator;
+    weight_function_ = scale_estimator == UnitScale ? UnitWeight : weight_function;
   }
   // sparse_img_align.cpp:43-75
   size_t run(FramePtr ref_frame, FramePtr cur_frame) {
@@ -329,6 +342,7 @@ class SparseImgAlign {
     svo_b200_sia_stats st;
     visible_fts_.assign(n, 0);
     Context& c = ref_frame->context();
+    c.check(svo_b200_sia_robust(c.get(), scale_estimator_, weight_function_));  // this object's mode, set on every call
     c.check(svo_b200_sparse_img_align(c.get(), ref_frame->device(), cur_frame->device(), &cam, &opt, T_cur_from_ref.m,
                                       px.data(), f.data(), pos.data(), has_point.data(), ref_pos.data(), (int)n,
                                       visible_fts_.data(), H_.data(), &st, nullptr, 0, nullptr));
@@ -346,6 +360,7 @@ class SparseImgAlign {
 
  private:
   int max_level_, min_level_, n_iter_;
+  int scale_estimator_ = UnitScale, weight_function_ = UnitWeight;
   Matrix6d H_;
   std::vector<uint8_t> visible_fts_;
 };
