@@ -1608,6 +1608,23 @@ __global__ void __launch_bounds__(kSiaRobustThreads, 1) sia_robust_kernel(const 
   const double* b_pos = b_f + 3 * np;
   const uint8_t* b_hp = reinterpret_cast<const uint8_t*>(b_pos + 3 * np);
 
+  // No features: run() returns before it touches anything (:47-51), as svo_b200_sparse_img_align does without a launch --
+  // the pose exactly as given (no quaternion round trip), H and the stats 0, no level run (scales NaN).  N is the same in
+  // every thread of the CTA, so the whole CTA leaves before its first barrier.
+  if (N == 0) {
+    if (leader) {
+      if (P.T_out)
+        for (int k = 0; k < 12; ++k) P.T_out[12 * (size_t)pair + k] = job.T[k];
+      if (P.H_out)
+        for (int k = 0; k < 36; ++k) P.H_out[36 * (size_t)pair + k] = 0.0;
+      if (P.stats) P.stats[pair] = svo_b200_sia_stats{};
+      if (RP.scales_out)
+        for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) RP.scales_out[(size_t)pair * SVO_B200_MAX_LEVELS + l] = __int_as_float(0x7fc00000);
+      if (P.n_trace) *P.n_trace = 0;
+    }
+    return;
+  }
+
   // xyz_ref = f * |pos - ref_pos| (:107-108), as sia_kernel forms it
   for (int i = tid; i < N; i += T) {
     const double dxp = b_pos[3 * i] - job.ref_pos[0], dyp = b_pos[3 * i + 1] - job.ref_pos[1], dzp = b_pos[3 * i + 2] - job.ref_pos[2];
@@ -1751,8 +1768,10 @@ __global__ void __launch_bounds__(kSiaRobustThreads, 1) sia_robust_kernel(const 
           for (int w = 0; w < kSiaRobustWarps; ++w) n += s.cnt[w];
           if (leader) s.n_pre = n;
           n_meas_pre += (long long)n * kPatchArea;
-          // getMedian of no errors is undefined in the reference: scale_ stays (not pinned)
-          if (n == 0 || !want_scale) break;
+          // getMedian of no errors is undefined in the reference: scale_ stays (not pinned).  n is the same in every thread;
+          // the barrier keeps s.cnt from being rewritten (the first pass below, or the next level's precompute when n_iter
+          // is 0) before every warp has read it here
+          if (n == 0 || !want_scale) { __syncthreads(); break; }
           kth = n * kPatchArea / 2;  // vk::getMedian: nth_element at floor(n / 2)
         }
         if (warp == 0) {  // lane l scans bins [8 l, 8 l + 8)

@@ -15,7 +15,8 @@ from tests import sia_robust_cases as rc
 pytestmark = pytest.mark.gpu
 
 NAMES = [k["name"] for k in rc.cases()]
-POSE_TOL = 1e-4
+POSE_TOL = 1e-9  # observed on an H100 (NVIDIA H100 80GB HBM3): 1.1e-13 m (occluded_unit)
+CHI2_RTOL = 5e-5  # trace chi2, relative: serial f32 sum vs per-patch f32 then f64 (observed up to 5.0e-6)
 KSIA_THREADS = {96, 160, 320, 384, 512}  # block sizes of sia_kernel's instantiations (the robust kernel runs 256)
 
 
@@ -40,7 +41,8 @@ def gpu_run(ctx, k, weight=None, scale=capi.SCALE_MAD, frames=None):
 @pytest.mark.parametrize("name", NAMES)
 def test_robust_single_call_equals_oracle(ctx, oracle, name):
     """Mask and n_tracked exact; the scale bit for bit where it comes from the initial pose (the first level) and within
-    1e-5 relative where a later level recomputed it; the accept / reject sequence of the trace equal; pose within 1e-4."""
+    1e-5 relative where a later level recomputed it; the trace's (level, iter, accepted, n_meas) equal and its chi2 within
+    CHI2_RTOL; pose within POSE_TOL."""
     k = rc.case(name)
     o = rc.oracle_run(k)
     g = gpu_run(ctx, k)
@@ -58,7 +60,11 @@ def test_robust_single_call_equals_oracle(ctx, oracle, name):
     assert g["n_tracked"] == o["n_tracked"], (g["n_tracked"], o["n_tracked"])
     for l in range(k["min_level"], k["max_level"]):
         assert s[l] == o["scales"][l] or abs(s[l] - o["scales"][l]) <= 1e-5 * abs(o["scales"][l]), (l, s, o["scales"])
-    assert [(t["level"], t["iter"], t["accepted"]) for t in g["trace"]] == [(t["level"], t["iter"], t["accepted"]) for t in o["trace"]]
+    assert [(t["level"], t["iter"], t["accepted"], t["n_meas"]) for t in g["trace"]] == \
+        [(t["level"], t["iter"], t["accepted"], t["n_meas"]) for t in o["trace"]]
+    for a, b in zip(g["trace"], o["trace"]):
+        assert (np.isnan(a["chi2"]) and np.isnan(b["chi2"])) or abs(a["chi2"] - b["chi2"]) <= CHI2_RTOL * abs(b["chi2"]), \
+            (a["chi2"], b["chi2"])
     dt, dr = synth.pose_error(g["T"], o["T"])
     print(f"{name}: |dt| {dt:.2e} m, dR {dr:.2e} rad vs oracle")
     assert dt <= POSE_TOL and dr <= POSE_TOL, (dt, dr)
