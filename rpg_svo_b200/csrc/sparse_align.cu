@@ -353,6 +353,19 @@ __device__ __forceinline__ double h_chunk_value(const double (&a)[6], const doub
   else if constexpr (IDX == 21) return cnt;
   else return 0.0;
 }
+// one feature's contribution to the 8 values of chunk CH
+template <int CH>
+__device__ __forceinline__ void h_chunk_add(double (&v)[8], const double (&a)[6], const double (&b)[6], double sxx, double sxy,
+                                            double syy, double cnt) {
+  v[0] += h_chunk_value<CH, 0>(a, b, sxx, sxy, syy, cnt);
+  v[1] += h_chunk_value<CH, 1>(a, b, sxx, sxy, syy, cnt);
+  v[2] += h_chunk_value<CH, 2>(a, b, sxx, sxy, syy, cnt);
+  v[3] += h_chunk_value<CH, 3>(a, b, sxx, sxy, syy, cnt);
+  v[4] += h_chunk_value<CH, 4>(a, b, sxx, sxy, syy, cnt);
+  v[5] += h_chunk_value<CH, 5>(a, b, sxx, sxy, syy, cnt);
+  v[6] += h_chunk_value<CH, 6>(a, b, sxx, sxy, syy, cnt);
+  v[7] += h_chunk_value<CH, 7>(a, b, sxx, sxy, syy, cnt);
+}
 
 // ---- cluster helpers (CS == 1: plain CTA, everything below folds to local shared memory) ------------
 __device__ __forceinline__ unsigned cluster_rank() {
@@ -455,38 +468,62 @@ __device__ __forceinline__ void xg_allreduce(const XgParams& X, int pair, unsign
 
 // Per-warp part of the H reduction: the 24 values (21 unique entries of sum_f Sxx aa^T + Sxy (ab^T + ba^T) + Syy bb^T, the
 // feature count, two pads) of this warp's features, into dst[0..23] (shared memory): three transposed 8-value warp
-// reductions computed chunk by chunk so that only ~8 accumulators are live at a time.
-// `get(k, x, y, zi, sxx, sxy, syy, cnt)` yields feature k's data.
+// reductions.  `get(k, x, y, zi, sxx, sxy, syy, cnt)` yields feature k's data.
+// ROLL (throughput geometry): ONE loop over the thread's features (a loop, not FPT copies: instruction-cache footprint), each
+// feature's data and Jacobian rows formed once and added to all 24 accumulators.  Otherwise the sums are computed chunk by
+// chunk, the loop unrolled, so that only ~8 accumulators are live at a time.  Every accumulator sees the same operands in
+// the same order (feature 0, 1, ...) either way, so the partials are bit-identical.
 template <int FPT, bool ROLL, class Get>
 __device__ __forceinline__ void warp_h_partials(Get get, double* dst) {
   const int lane = threadIdx.x & 31;
-  auto do_chunk = [&](auto chunk_tag) {
-    constexpr int CH = decltype(chunk_tag)::value;
-    double v[8];
+  if constexpr (ROLL) {
+    double v0[8], v1[8], v2[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = 0.0;
-#pragma unroll(ROLL ? 1 : FPT)
-    for (int k = 0; k < FPT; ++k) {  // ROLL: a loop, not FPT copies (instruction-cache footprint of the throughput geometry)
+    for (int j = 0; j < 8; ++j) v0[j] = v1[j] = v2[j] = 0.0;
+#pragma unroll 1
+    for (int k = 0; k < FPT; ++k) {
       double x, y, zi, sxx, sxy, syy, cnt;
       get(k, x, y, zi, sxx, sxy, syy, cnt);
       double a[6], b[6];
       jac_rows(x, y, zi, a, b);
-      v[0] += h_chunk_value<CH, 0>(a, b, sxx, sxy, syy, cnt);
-      v[1] += h_chunk_value<CH, 1>(a, b, sxx, sxy, syy, cnt);
-      v[2] += h_chunk_value<CH, 2>(a, b, sxx, sxy, syy, cnt);
-      v[3] += h_chunk_value<CH, 3>(a, b, sxx, sxy, syy, cnt);
-      v[4] += h_chunk_value<CH, 4>(a, b, sxx, sxy, syy, cnt);
-      v[5] += h_chunk_value<CH, 5>(a, b, sxx, sxy, syy, cnt);
-      v[6] += h_chunk_value<CH, 6>(a, b, sxx, sxy, syy, cnt);
-      v[7] += h_chunk_value<CH, 7>(a, b, sxx, sxy, syy, cnt);
+      h_chunk_add<0>(v0, a, b, sxx, sxy, syy, cnt);
+      h_chunk_add<1>(v1, a, b, sxx, sxy, syy, cnt);
+      h_chunk_add<2>(v2, a, b, sxx, sxy, syy, cnt);
     }
-    warp_reduce_t<8>(v);
-    if ((lane & 3) == 0) dst[CH * 8 + (lane >> 2)] = v[0];
-  };
-  do_chunk(std::integral_constant<int, 0>{});
-  do_chunk(std::integral_constant<int, 1>{});
-  do_chunk(std::integral_constant<int, 2>{});
+    warp_reduce_t<8>(v0);
+    if ((lane & 3) == 0) dst[lane >> 2] = v0[0];
+    warp_reduce_t<8>(v1);
+    if ((lane & 3) == 0) dst[8 + (lane >> 2)] = v1[0];
+    warp_reduce_t<8>(v2);
+    if ((lane & 3) == 0) dst[16 + (lane >> 2)] = v2[0];
+  } else {
+    auto do_chunk = [&](auto chunk_tag) {
+      constexpr int CH = decltype(chunk_tag)::value;
+      double v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = 0.0;
+#pragma unroll(FPT)
+      for (int k = 0; k < FPT; ++k) {
+        double x, y, zi, sxx, sxy, syy, cnt;
+        get(k, x, y, zi, sxx, sxy, syy, cnt);
+        double a[6], b[6];
+        jac_rows(x, y, zi, a, b);
+        h_chunk_add<CH>(v, a, b, sxx, sxy, syy, cnt);
+      }
+      warp_reduce_t<8>(v);
+      if ((lane & 3) == 0) dst[CH * 8 + (lane >> 2)] = v[0];
+    };
+    do_chunk(std::integral_constant<int, 0>{});
+    do_chunk(std::integral_constant<int, 1>{});
+    do_chunk(std::integral_constant<int, 2>{});
+  }
 }
+
+// Named barrier `id` (not 0, which __syncthreads uses) of `n` threads: bar.arrive releases this thread's prior shared-memory
+// writes to the threads that bar.sync on it and does not wait; bar.sync waits until all n have arrived.
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+constexpr int kHsumBarrier = 1;  // the level's H partials (one CTA per pair)
 
 // Sum of the 21 unique H entries + one count over the per-feature moments of the whole pair, once per level
 // (and in the rare "slow path"): per-warp partials, one shared-memory hop, warp 0 adds the per-warp partials (and, in the
@@ -494,11 +531,22 @@ __device__ __forceinline__ void warp_h_partials(Get get, double* dst) {
 // s.sums[0..23] of EVERY CTA of the pair, visible to warp 0 only (callers that need them elsewhere synchronise).
 // (`sum_warp`: the warp that adds the per-warp partials and afterwards sees s.sums -- warp 0, or, one CTA per pair, another
 // warp of the caller's choice.)
-template <int FPT, int CS, bool XG, bool ROLL, class SH, class Get>
+// ARRIVE (one CTA per pair): the other warps do not wait for the sum -- they arrive on a named barrier after writing their
+// partials and return at once; only `sum_warp` waits on it.  The caller must keep s.hpart from being rewritten, and the
+// barrier from being arrived on again, until `sum_warp` has summed (a block barrier that `sum_warp` reaches after it).
+template <int FPT, int CS, bool XG, bool ROLL, class SH, bool ARRIVE = false, class Get>
 __device__ __forceinline__ void pair_sum_h_to_warp0(Get get, SH& s, int nwarps, const XgParams& xg, int xg_pair, int sum_warp = 0) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   warp_h_partials<FPT, ROLL>(get, &s.hpart[warp * kPartK]);
-  __syncthreads();
+  if constexpr (CS == 1 && ARRIVE) {
+    if (warp != sum_warp) {
+      named_bar_arrive(kHsumBarrier, nwarps * 32);
+      return;
+    }
+    named_bar_sync(kHsumBarrier, nwarps * 32);
+  } else {
+    __syncthreads();
+  }
   if constexpr (CS == 1) {
     if (warp == sum_warp) {
       double acc = 0.0;
@@ -833,6 +881,9 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     s.tk[4] = clock64();
 #endif
     for (int k = 0; k < 36; ++k) s.Hs[k] = 0.0;
+    // tiled copy of the running level's current image, read by the residual passes: the first level's here, every further
+    // one at the end of the level before it
+    if (TL) s.cur_tl = reinterpret_cast<const uint4*>(job.cur_tl[EVAL ? P.eval_level : P.max_level]);
   }
   __syncthreads();
   mbar_wait(&s.mbar, 0);
@@ -980,30 +1031,31 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       }
     }
   };
-  // ---- gradient moments Sxx, Sxy, Syy of this thread's patches in `mask` (zero for the others), summed pixel by pixel from
-  //      the gradient array pd in shared memory
+  // ---- gradient moments Sxx, Sxy, Syy of feature k of this thread if it is in `mask` (else zero), summed pixel by pixel
+  //      from the gradient array pd in shared memory; patch_moments: of all its features
+  auto feat_moments = [&](const float2* pd, const unsigned mask, const int k, double& sxx, double& sxy, double& syy) {
+    sxx = sxy = syy = 0.0;
+    if (!((mask >> k) & 1u)) return;
+    const int slot = tid + k * T;
+#pragma unroll
+    for (int p = 0; p < kPatchArea; ++p) {
+      const float2 gr = pd[p * SA + slot];
+      const double dx = (double)gr.x, dy = (double)gr.y;
+      sxx = fma(dx, dx, sxx);
+      sxy = fma(dx, dy, sxy);
+      syy = fma(dy, dy, syy);
+    }
+  };
   auto patch_moments = [&](const float2* pd, const unsigned mask, double (&sxx)[FPT], double (&sxy)[FPT], double (&syy)[FPT]) {
 #pragma unroll
-    for (int k = 0; k < FPT; ++k) {
-      sxx[k] = sxy[k] = syy[k] = 0.0;
-      if (!((mask >> k) & 1u)) continue;
-      const int slot = tid + k * T;
-#pragma unroll
-      for (int p = 0; p < kPatchArea; ++p) {
-        const float2 gr = pd[p * SA + slot];
-        const double dx = (double)gr.x, dy = (double)gr.y;
-        sxx[k] = fma(dx, dx, sxx[k]);
-        sxy[k] = fma(dx, dy, sxy[k]);
-        syy[k] = fma(dy, dy, syy[k]);
-      }
-    }
+    for (int k = 0; k < FPT; ++k) feat_moments(pd, mask, k, sxx[k], sxy[k], syy[k]);
   };
   // ---- precomputeReferencePatches (:84-145) of one level into the patch arrays (pr, pd): visibility bits, the f32 patch and
   //      its gradients, and the per-feature gradient moments m_* the H reduction needs.  `with_windows`: also request the
   //      current-image windows (between the footprint loads and the arithmetic, so that both latencies overlap).
   //      Throughput geometry: the loop over the thread's features is not unrolled, so moments stored here would be indexed by
   //      the feature and live in local memory, which misses the small L1 left beside 3 x 75 KB of shared memory; it leaves
-  //      m_* alone and the caller sums them afterwards with patch_moments(pd, vis_mask) -- a visible patch has its gradients
+  //      m_* alone and the H sum takes them from pd with feat_moments(pd, vis_mask) -- a visible patch has its gradients
   //      in pd (zero for a stale one), summed in the same order.  The other geometries unroll the loop and keep the moments of
   //      the patch arithmetic (a second pass over pd would lengthen the latency path of the cluster geometries).
   auto level_patches = [&](const int level, float* pr, float2* pd, const float* pr_stale, const int mode, const bool with_windows,
@@ -1162,8 +1214,6 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       tma_bulk_g2s(stage, cur_img, img_bytes, &s.mbar);
     }
     if (cta_leader) s.st[g & 1u].old_model = s.st[g & 1u].model;  // optimizeGaussNewton: ModelType old_model(model) [EXT]
-    // read by the residual passes, after the barriers of the level setup
-    if (TL && cta_leader) s.cur_tl = reinterpret_cast<const uint4*>(job.cur_tl[level]);
     // next level: pull its current image (coarse levels, staged whole) into L2 while this level iterates
     if (tid == 0 && crank == 0 && level > lvl_lo) {
       const uint32_t nb = ((uint32_t)(P.w[level - 1] * P.h[level - 1]) + 15u) & ~15u;
@@ -1181,11 +1231,18 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       //      between the footprint loads and the patch arithmetic
       double m_sxx[FPT], m_sxy[FPT], m_syy[FPT];
       level_patches(level, pat_ref, pat_dxy, (const float*)nullptr, mode, true, m_sxx, m_sxy, m_syy);
-      if constexpr (SS) patch_moments(pat_dxy, vis_mask, m_sxx, m_sxy, m_syy);
       SIA_DBG(if ((SVO_SIA_DEBUG && P.debug) && tid == 0) { tq1 = clock64(); s.tk[7] += tq1 - tq0; })
-      pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
+      // Only fwarp waits for the other warps' H partials (!EVAL: a named barrier the others arrive on and pass).  fwarp
+      // reads s.hpart before it reaches barrier A of iteration 0, and nothing rewrites s.hpart -- the slow path's sum, the
+      // next level's partials -- or arrives on the named barrier again before every warp has passed that barrier A
+      // (n_iter == 0: the barrier at the end of the level).  sum_vis is fwarp's alone until the outputs.  EVAL keeps the block
+      // barrier: it runs one pass of one level.
+      pair_sum_h_to_warp0<FPT, CS, XG, SS, SH, !EVAL>(
           [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
-            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = sel_k(m_sxx, k); sxy = sel_k(m_sxy, k); syy = sel_k(m_syy, k); cnt = ((vis_mask >> k) & 1u) ? 1.0 : 0.0;
+            { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); }
+            if constexpr (SS) feat_moments(pat_dxy, vis_mask, k, sxx, sxy, syy);
+            else { sxx = sel_k(m_sxx, k); sxy = sel_k(m_sxy, k); syy = sel_k(m_syy, k); }
+            cnt = ((vis_mask >> k) & 1u) ? 1.0 : 0.0;
             // opaque to the optimiser: otherwise the level-invariant Jacobian rows are hoisted out of the level loop and
             // parked in local memory (17 doubles per thread, written once and re-read every level)
             asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));
@@ -1376,10 +1433,13 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       // contributed in this pass ("slow path"; all threads, one block barrier inside)
       auto slow_sum_h = [&]() {
         double q_sxx[FPT], q_sxy[FPT], q_syy[FPT];
-        patch_moments(pat_dxy, in_mask, q_sxx, q_sxy, q_syy);
+        if constexpr (!SS) patch_moments(pat_dxy, in_mask, q_sxx, q_sxy, q_syy);
         pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
             [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
-              { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); } sxx = sel_k(q_sxx, k); sxy = sel_k(q_sxy, k); syy = sel_k(q_syy, k); cnt = 0.0;
+              { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); }
+              if constexpr (SS) feat_moments(pat_dxy, in_mask, k, sxx, sxy, syy);
+              else { sxx = sel_k(q_sxx, k); sxy = sel_k(q_sxy, k); syy = sel_k(q_syy, k); }
+              cnt = 0.0;
               asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));  // see the per-level call: no hoisting into local memory
             },
             s, nwarps, P.xg, pair);
@@ -1498,9 +1558,15 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     }
     // stage region / patches are rewritten by the next level; the leader's state writes are visible.  Upfront variant: only
     // CTA-local buffers are reused between levels (every level has its own patch arrays, the exchange buffers alternate by
-    // the parity of the running iteration counter), so the CTAs of the pair need not meet here
-    if constexpr (UP) __syncthreads();
-    else pair_sync<CS>();
+    // the parity of the running iteration counter), so the CTAs of the pair need not meet here.
+    // One CTA per pair: the barrier publishes the next level's s.cur_tl -- the warps that do not sum the level's H reach its
+    // first residual pass without another barrier -- and, when n_iter == 0, orders the H sum against the next level's.
+    if constexpr (UP) {
+      __syncthreads();
+    } else {
+      if (TL && cta_leader && level > lvl_lo) s.cur_tl = reinterpret_cast<const uint4*>(job.cur_tl[level - 1]);
+      pair_sync<CS>();
+    }
   }
   if constexpr (UP) pair_sync<CS>();  // no CTA of the cluster exits while another may still write into its shared memory
 

@@ -17,7 +17,7 @@ def find(s):
 marks = [("prologue", find("__global__ void __launch_bounds__(MAXT, MINB) sia_kernel")),
          ("level_setup", find("for (int level = lvl_hi; level >= lvl_lo; --level)")),
          ("precompute", find("// ---- precomputeReferencePatches")),
-         ("hsum+factor", find("pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(")),
+         ("hsum+factor", find("pair_sum_h_to_warp0<FPT, CS, XG, SS, SH")),
          ("pass", find("// ---- Gauss-Newton iterations at this level")),
          ("reduce", find("// ---- pair-wide sums: per-warp transposed reduction")),
          ("tail", find("SIA_DBG(long long ti2 = 0;)")),
