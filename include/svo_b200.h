@@ -15,6 +15,8 @@
  *   svo_b200_depth_filter_update    <- DepthFilter::updateSeeds               svo/include/svo/depth_filter.h:155
  *                                      (Matcher::findEpipolarMatchDirect, updateSeed, computeTau inside)
  *   svo_b200_frame_*                <- svo::Frame image pyramid               svo/include/svo/frame.h:52, svo/src/frame.cpp:156-165
+ *   svo_b200_klt_*                  <- initialization::trackKlt's             svo/src/initialization.cpp:127-169
+ *                                      cv::calcOpticalFlowPyrLK
  *
  * Conventions
  *   - every function returns 0 on success, a negative SVO_B200_E* code on argument / CUDA errors;
@@ -448,6 +450,57 @@ int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_b200_frame*
                                         double* depth_out, double* px_cur_out /*M*2*/, int* search_level_out,
                                         double* epi_length_out, uint8_t* reject_out, double* A_cur_ref_out /*M*4*/,
                                         int* n_zmssd_out);
+
+/* ------------------------------------------------------------------ KLT tracking of the two-view initialisation ------ */
+/* initialization::trackKlt (svo/src/initialization.cpp:127-169) tracks every corner of the first keyframe into each new
+ * frame with cv::calcOpticalFlowPyrLK(ref, cur, px_ref, px_cur, status, err, Size(30, 30), 4,
+ * TermCriteria(COUNT + EPS, 30, 0.001), OPTFLOW_USE_INITIAL_FLOW).  These entry points run OpenCV's published algorithm
+ * ([EXT] modules/video/src/lkpyramid.cpp) on the device; see DESIGN.md section 4.2d for the rules it follows.
+ *
+ * An LK pyramid is OpenCV's, not the frame's vk::halfSample pyramid: level l+1 = pyrDown(level l) ([1 4 6 4 1] filter,
+ * reflect-101 borders, (sum + 128) >> 8, size ((w+1)/2, (h+1)/2)), and levels stop once the next one would be no larger
+ * than the 30-pixel window (640 x 480 and 752 x 480 get 4 levels, 644 x 484 gets 5).  The pyramid of the previous image
+ * also holds the Scharr derivatives of every level (interleaved int16 dx, dy; zero outside the level).  Build the
+ * reference frame's pyramid once with derivatives and reuse it; each new frame needs its own pyramid without. */
+typedef struct svo_b200_klt_pyramid svo_b200_klt_pyramid;
+int svo_b200_klt_pyramid_create(svo_b200_ctx* ctx, svo_b200_klt_pyramid** pyr_out);
+void svo_b200_klt_pyramid_destroy(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr);
+/* Builds the pyramid (at most max_level + 1 levels) from level 0 of `frame`, already on the device.  with_derivatives:
+ * 1 = also the Scharr derivatives (the previous image of svo_b200_klt_track), 0 = images only. */
+int svo_b200_klt_pyramid_build(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr, const svo_b200_frame* frame, int max_level,
+                               int with_derivatives);
+/* Number of levels the last build made (0 before the first). */
+int svo_b200_klt_pyramid_levels(const svo_b200_klt_pyramid* pyr);
+/* Copies one level out: img_out w*h bytes, deriv_out w*h*2 int16 (interleaved dx, dy; needs a build with derivatives);
+ * either may be NULL. */
+int svo_b200_klt_pyramid_download(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* pyr, int level, uint8_t* img_out,
+                                  int16_t* deriv_out);
+
+typedef struct {
+  int win_size;  /* only the reference's 30 is supported */
+  int max_level; /* coarsest level (initialization.cpp: 4); the levels used are min(max_level + 1, levels of both pyramids) */
+  int max_iter;  /* iterations per level (30), clamped to [0, 100] as OpenCV does */
+  double eps;    /* stop when |delta| <= eps (0.001), clamped to [0, 10] as OpenCV does */
+} svo_b200_klt_options;
+/* How a point's tracking ended at a level. */
+#define SVO_B200_KLT_CONVERGED 0     /* delta . delta <= eps^2 */
+#define SVO_B200_KLT_HALF_STEP 1     /* two consecutive steps nearly cancelled: stepped back half a step */
+#define SVO_B200_KLT_MAX_ITER 2      /* max_iter steps taken */
+#define SVO_B200_KLT_OUT_OF_BOUNDS 3 /* the window left the level (status 0 only at level 0) */
+#define SVO_B200_KLT_SMALL_EIG 4     /* min eigenvalue of the window's gradient matrix / 900 < 1e-4, or its determinant
+                                        < FLT_EPSILON (status 0 only at level 0) */
+typedef struct {
+  int32_t reason;                              /* SVO_B200_KLT_* at level 0 */
+  int32_t level_reason[SVO_B200_MAX_LEVELS];   /* SVO_B200_KLT_* per level, -1 for levels not run */
+  int32_t iters[SVO_B200_MAX_LEVELS];          /* steps taken per level */
+} svo_b200_klt_exit;
+/* calcOpticalFlowPyrLK with OPTFLOW_USE_INITIAL_FLOW for N points: prev_pts N*2 floats; next_pts_io N*2 floats, in = the
+ * initial guess, out = the tracked points; status_out N bytes (1 tracked, 0 lost); exit_out (N entries) may be NULL.
+ * OpenCV's `err` output is not produced.  `prev` must have been built with derivatives, `next` with or without; both from
+ * frames of one size.  N == 0 returns 0. */
+int svo_b200_klt_track(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* prev, const svo_b200_klt_pyramid* next,
+                       const svo_b200_klt_options* opt, int N, const float* prev_pts, float* next_pts_io, uint8_t* status_out,
+                       svo_b200_klt_exit* exit_out);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsvo_b200.so")
-SOURCES = ["context.cu", "sparse_align.cu", "align.cu", "pose_opt.cu", "depth_filter.cu", "reproject.cu", "detect.cu"]
+SOURCES = ["context.cu", "sparse_align.cu", "align.cu", "pose_opt.cu", "depth_filter.cu", "reproject.cu", "detect.cu", "klt.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false",
               "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-cudart", "static"]
 

@@ -95,6 +95,13 @@ def load() -> C.CDLL:
         _lib.svo_b200_frame_pool_get.argtypes = [C.c_void_p, C.c_int]
         _lib.svo_b200_frame_pool_get.restype = C.c_void_p
         _lib.svo_b200_destroy.restype = None
+        _lib.svo_b200_klt_pyramid_destroy.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.svo_b200_klt_pyramid_destroy.restype = None
+        _lib.svo_b200_klt_pyramid_build.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+        _lib.svo_b200_klt_pyramid_levels.argtypes = [C.c_void_p]
+        _lib.svo_b200_klt_pyramid_download.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        _lib.svo_b200_klt_track.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -625,3 +632,80 @@ def _fast_detect(self, frame: Frame, cell_size, n_pyr_levels, detection_threshol
 
 
 Context.fast_detect = _fast_detect
+
+
+# ------------------------------------------------------------------ KLT tracking of the two-view initialisation
+KLT_CONVERGED, KLT_HALF_STEP, KLT_MAX_ITER, KLT_OUT_OF_BOUNDS, KLT_SMALL_EIG = 0, 1, 2, 3, 4  # SVO_B200_KLT_*
+
+
+class KltOptions(C.Structure):
+    _fields_ = [("win_size", C.c_int), ("max_level", C.c_int), ("max_iter", C.c_int), ("eps", C.c_double)]
+
+
+class KltExit(C.Structure):
+    _fields_ = [("reason", C.c_int32), ("level_reason", C.c_int32 * MAX_LEVELS), ("iters", C.c_int32 * MAX_LEVELS)]
+
+
+class KltPyramid:
+    """OpenCV's LK pyramid of one frame's level 0 (and, for the previous image, its Scharr derivatives) in HBM."""
+
+    def __init__(self, ctx: "Context"):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx._check(ctx.lib.svo_b200_klt_pyramid_create(ctx.h, C.byref(h)))
+        self.h = h
+
+    def build(self, frame: Frame, derivatives: bool, max_level: int = 4) -> "KltPyramid":
+        self.ctx._check(self.ctx.lib.svo_b200_klt_pyramid_build(self.ctx.h, self.h, frame.h, int(max_level), int(bool(derivatives))))
+        self.width, self.height = frame.width, frame.height
+        return self
+
+    @property
+    def n_levels(self) -> int:
+        return int(self.ctx.lib.svo_b200_klt_pyramid_levels(self.h))
+
+    def download(self, level: int, derivatives: bool = False):
+        """(image h x w uint8, derivatives h x w x 2 int16 or None) of one level."""
+        lib = self.ctx.lib
+        w, h = self.width, self.height  # level l is ((w+1)/2, (h+1)/2) of level l-1
+        for _ in range(level):
+            w, h = (w + 1) // 2, (h + 1) // 2
+        img = np.zeros((h, w), np.uint8)
+        der = np.zeros((h, w, 2), np.int16) if derivatives else None
+        self.ctx._check(lib.svo_b200_klt_pyramid_download(self.ctx.h, self.h, int(level), _p(img), _p(der)))
+        return img, der
+
+    def destroy(self):
+        if self.h:
+            self.ctx.lib.svo_b200_klt_pyramid_destroy(self.ctx.h, self.h)
+            self.h = None
+
+
+def _klt_pyramid(self, frame: Frame, derivatives: bool, max_level: int = 4) -> KltPyramid:
+    """The LK pyramid of `frame`'s level 0 (already on the device), with the Scharr derivatives if `derivatives`."""
+    return KltPyramid(self).build(frame, derivatives, max_level)
+
+
+def _klt_track(self, prev: KltPyramid | None, nxt: KltPyramid | None, prev_pts, next_pts, max_level=4, max_iter=30, eps=0.001,
+               win_size=30, want_exit=True):
+    """calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, ..., OPTFLOW_USE_INITIAL_FLOW) on the device.
+    dict(next_pts (N x 2 float32), status (N uint8), and with want_exit: reason (N), level_reason / iters (N x MAX_LEVELS))."""
+    lib = self.lib
+    p0 = np.ascontiguousarray(prev_pts, np.float32).reshape(-1, 2)
+    p1 = np.ascontiguousarray(next_pts, np.float32).reshape(-1, 2).copy()
+    n = len(p0)
+    st = np.zeros(max(n, 1), np.uint8)
+    ex = (KltExit * max(n, 1))() if want_exit else None
+    opt = KltOptions(int(win_size), int(max_level), int(max_iter), float(eps))
+    self._check(lib.svo_b200_klt_track(self.h, prev.h if prev is not None else None, nxt.h if nxt is not None else None,
+                                       C.byref(opt), n, _p(p0), _p(p1), _p(st), ex))
+    o = dict(next_pts=p1, status=st[:n])
+    if want_exit:
+        o["reason"] = np.array([e.reason for e in ex[:n]], np.int32)
+        o["level_reason"] = np.array([list(e.level_reason) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
+        o["iters"] = np.array([list(e.iters) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
+    return o
+
+
+Context.klt_pyramid = _klt_pyramid
+Context.klt_track = _klt_track

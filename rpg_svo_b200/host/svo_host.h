@@ -230,6 +230,7 @@ class Frame {
   }
   ~Frame() {
     for (Feature* f : fts_) delete f;  // frame.cpp:43-46
+    svo_b200_klt_pyramid_destroy(ctx_.get(), klt_);
     svo_b200_frame_destroy(ctx_.get(), dev_);
   }
   Frame(const Frame&) = delete;
@@ -245,12 +246,27 @@ class Frame {
                             m[8] * xyz_w[0] + m[9] * xyz_w[1] + m[10] * xyz_w[2] + m[11]});
   }
   size_t nObs() const { return fts_.size(); }
+  Vector3d c2f(double x, double y) const { return cam_->cam2world({x, y}); }  // frame.h:94
   svo_b200_frame* device() const { return dev_; }
   Context& context() const { return ctx_; }
+  // The LK pyramid cv::calcOpticalFlowPyrLK builds from img_pyr_[0] (initialization::trackKlt), built on first use and
+  // kept: the first keyframe's, with derivatives, serves every frame of the initialisation.
+  const svo_b200_klt_pyramid* kltPyramid(bool derivatives) {
+    if (!klt_) ctx_.check(svo_b200_klt_pyramid_create(ctx_.get(), &klt_));
+    if (klt_levels_ == 0 || (derivatives && !klt_derivs_)) {
+      ctx_.check(svo_b200_klt_pyramid_build(ctx_.get(), klt_, dev_, 4, derivatives ? 1 : 0));
+      klt_levels_ = svo_b200_klt_pyramid_levels(klt_);
+      klt_derivs_ = derivatives;
+    }
+    return klt_;
+  }
 
  private:
   Context& ctx_;
   svo_b200_frame* dev_ = nullptr;
+  svo_b200_klt_pyramid* klt_ = nullptr;
+  int klt_levels_ = 0;
+  bool klt_derivs_ = false;
 };
 typedef std::shared_ptr<Frame> FramePtr;
 
@@ -537,6 +553,65 @@ class FastDetector : public AbstractDetector {
   }
 };
 }  // namespace feature_detection
+
+// ------------------------------------------------------------------------------------------------
+// svo::initialization (svo/src/initialization.cpp:107-169): the per-frame work of KltHomographyInit.  cv::Point2f is
+// restated as Point2f; the KLT tracker runs on the device (svo_b200_klt_track).
+// ------------------------------------------------------------------------------------------------
+struct Point2f {
+  float x, y;
+};
+struct Config {  // the values of svo/src/config.cpp that the initialisation reads
+  static int gridSize() { return 30; }
+  static int nPyrLevels() { return 3; }
+  static double triangMinCornerScore() { return 20.0; }
+};
+
+namespace initialization {
+inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, std::vector<Vector3d>& f_vec) {  // :107-125
+  Features new_features;
+  feature_detection::FastDetector detector(frame->img_pyr_[0].cols, frame->img_pyr_[0].rows, Config::gridSize(), Config::nPyrLevels());
+  detector.detect(frame.get(), Config::triangMinCornerScore(), new_features);
+  px_vec.clear(); px_vec.reserve(new_features.size());
+  f_vec.clear(); f_vec.reserve(new_features.size());
+  for (Feature* ftr : new_features) {
+    px_vec.push_back(Point2f{(float)ftr->px[0], (float)ftr->px[1]});
+    f_vec.push_back(ftr->f);
+    delete ftr;
+  }
+}
+
+// calcOpticalFlowPyrLK(ref, cur, px_ref, px_cur, ..., Size(30, 30), 4, (COUNT + EPS, 30, 0.001), OPTFLOW_USE_INITIAL_FLOW),
+// then lost points erased from px_ref, px_cur and f_ref in order; f_cur and the disparities of the rest (:127-169).
+inline void trackKlt(const FramePtr& frame_ref, const FramePtr& frame_cur, std::vector<Point2f>& px_ref, std::vector<Point2f>& px_cur,
+                     std::vector<Vector3d>& f_ref, std::vector<Vector3d>& f_cur, std::vector<double>& disparities) {
+  const svo_b200_klt_options opt = {30, 4, 30, 0.001};
+  std::vector<uint8_t> status(px_ref.size());
+  px_cur.resize(px_ref.size());  // the reference requires the initial flow to have px_ref's size
+  Context& c = frame_cur->context();
+  c.check(svo_b200_klt_track(c.get(), frame_ref->kltPyramid(true), frame_cur->kltPyramid(false), &opt, (int)px_ref.size(),
+                             reinterpret_cast<const float*>(px_ref.data()), reinterpret_cast<float*>(px_cur.data()), status.data(), nullptr));
+  auto px_ref_it = px_ref.begin();
+  auto px_cur_it = px_cur.begin();
+  auto f_ref_it = f_ref.begin();
+  f_cur.clear(); f_cur.reserve(px_cur.size());
+  disparities.clear(); disparities.reserve(px_cur.size());
+  for (size_t i = 0; px_ref_it != px_ref.end(); ++i) {
+    if (!status[i]) {
+      px_ref_it = px_ref.erase(px_ref_it);
+      px_cur_it = px_cur.erase(px_cur_it);
+      f_ref_it = f_ref.erase(f_ref_it);
+      continue;
+    }
+    f_cur.push_back(frame_cur->c2f(px_cur_it->x, px_cur_it->y));
+    const double dx = px_ref_it->x - px_cur_it->x, dy = px_ref_it->y - px_cur_it->y;  // float differences, widened
+    disparities.push_back(std::sqrt(dx * dx + dy * dy));
+    ++px_ref_it;
+    ++px_cur_it;
+    ++f_ref_it;
+  }
+}
+}  // namespace initialization
 
 struct Seed {
   static int& batch_counter() { static int c = 0; return c; }
