@@ -466,7 +466,10 @@ typedef struct svo_b200_klt_pyramid svo_b200_klt_pyramid;
 int svo_b200_klt_pyramid_create(svo_b200_ctx* ctx, svo_b200_klt_pyramid** pyr_out);
 void svo_b200_klt_pyramid_destroy(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr);
 /* Builds the pyramid (at most max_level + 1 levels) from level 0 of `frame`, already on the device.  with_derivatives:
- * 1 = also the Scharr derivatives (the previous image of svo_b200_klt_track), 0 = images only. */
+ * 1 = also the Scharr derivatives (the previous image of svo_b200_klt_track), 0 = images only.  A handle may be rebuilt
+ * at any size; it keeps its allocation where the new pyramid fits.  Returns SVO_B200_EINVAL for max_level < 0, and where
+ * OpenCV's cut would build more than SVO_B200_MAX_LEVELS levels (a side of 7681 pixels or more at max_level >= 8): such
+ * a pyramid is refused, not cut short, before anything is allocated or launched, and the handle keeps its last build. */
 int svo_b200_klt_pyramid_build(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr, const svo_b200_frame* frame, int max_level,
                                int with_derivatives);
 /* Number of levels the last build made (0 before the first). */
@@ -480,8 +483,9 @@ typedef struct {
   int win_size;  /* only the reference's 30 is supported */
   int max_level; /* coarsest level (initialization.cpp: 4); the levels used are min(max_level + 1, levels of both pyramids) */
   int max_iter;  /* iterations per level (30), clamped to [0, 100] as OpenCV does */
-  double eps;    /* stop when |delta| <= eps (0.001), clamped to [0, 10] as OpenCV does */
+  double eps;    /* stop when |delta| <= eps (0.001), clamped to at most 10 as OpenCV does */
 } svo_b200_klt_options;
+/* Unlike OpenCV, which clamps them, max_level < 0 and a negative or NaN eps return SVO_B200_EINVAL. */
 /* How a point's tracking ended at a level. */
 #define SVO_B200_KLT_CONVERGED 0     /* delta . delta <= eps^2 */
 #define SVO_B200_KLT_HALF_STEP 1     /* two consecutive steps nearly cancelled: stepped back half a step */
@@ -497,7 +501,9 @@ typedef struct {
 /* calcOpticalFlowPyrLK with OPTFLOW_USE_INITIAL_FLOW for N points: prev_pts N*2 floats; next_pts_io N*2 floats, in = the
  * initial guess, out = the tracked points; status_out N bytes (1 tracked, 0 lost); exit_out (N entries) may be NULL.
  * OpenCV's `err` output is not produced.  `prev` must have been built with derivatives, `next` with or without; both from
- * frames of one size.  N == 0 returns 0. */
+ * frames of one size (one handle may be both).  N == 0 returns 0.  prev_pts and next_pts_io may be the same buffer.  A
+ * point with a NaN, an infinite or a huge coordinate in prev_pts or in its guess is lost out of bounds at every level,
+ * as OpenCV loses it; its next_pts entry keeps the guess. */
 int svo_b200_klt_track(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* prev, const svo_b200_klt_pyramid* next,
                        const svo_b200_klt_options* opt, int N, const float* prev_pts, float* next_pts_io, uint8_t* status_out,
                        svo_b200_klt_exit* exit_out);

@@ -41,9 +41,12 @@ def lib() -> C.CDLL:
 
 
 def level_sizes(w, h, max_level=4, win=WIN):
-    """[(w, h)] of the LK pyramid's levels: buildOpticalFlowPyramid's level cut."""
+    """[(w, h)] of the LK pyramid's levels: buildOpticalFlowPyramid's level cut.  ValueError where the cut would build
+    more than MAX_LEVELS levels (svo_b200_klt_pyramid_build refuses those)."""
     ws, hs = np.zeros(MAX_LEVELS, np.int32), np.zeros(MAX_LEVELS, np.int32)
     n = lib().orc_klt_levels(w, h, max_level, win, _p(ws), _p(hs))
+    if n < 0:
+        raise ValueError(f"{w}x{h} at max_level {max_level}: more than {MAX_LEVELS} levels")
     return [(int(ws[i]), int(hs[i])) for i in range(n)]
 
 
@@ -68,6 +71,7 @@ def track(prev, nxt, prev_pts, next_pts, max_level=4, max_iter=30, eps=0.001, wi
     margins (N x MAX_LEVELS x 5: eps, half-step, eigenvalue, determinant, bounds; see orc_klt_track), n_levels)."""
     prev, nxt = np.ascontiguousarray(prev, np.uint8), np.ascontiguousarray(nxt, np.uint8)
     h, w = prev.shape
+    level_sizes(w, h, max_level, win)  # ValueError past MAX_LEVELS levels
     p0 = np.ascontiguousarray(prev_pts, np.float32).reshape(-1, 2)
     p1 = np.ascontiguousarray(next_pts, np.float32).reshape(-1, 2).copy()
     n = len(p0)

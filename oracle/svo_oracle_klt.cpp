@@ -9,8 +9,8 @@
 // its published algorithm:
 //   pyramid      level 0 = the image; level l+1 = pyrDown(level l): a separable [1 4 6 4 1] filter with reflect-101
 //                borders, even rows and columns kept, (sum + 128) >> 8; size ((w+1)/2, (h+1)/2).  Levels stop once the
-//                next one would be no larger than the window in either dimension.  Every level is read through a
-//                window-wide reflect-101 border.
+//                next one would be no larger than the window in either dimension; a cut past 8 levels is refused, as the
+//                device's build refuses it.  Every level is read through a window-wide reflect-101 border.
 //   derivatives  Scharr on every level of the previous image: dx = [-1 0 1] across of [3 10 3] down, dy = [3 10 3] across
 //                of [-1 0 1] down, reflect-101 borders, int16 pairs; zero outside the level.
 //   tracker      coarse to fine; half-window (win-1)/2; window corner floor(pt - halfWin); bilinear weights with 14 bits
@@ -24,11 +24,13 @@
 // pairwise halving (partial[i] + partial[i ^ 16], then ^ 8, ^ 4, ^ 2, ^ 1): one order fixed for the oracle and the kernel
 // alike, so that the two agree bit for bit.
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 namespace {
@@ -52,9 +54,11 @@ struct Padded {
   const int16_t* D(int x, int y) const { return der.data() + ((size_t)(y + B) * stride() + (x + B)) * 2; }
 };
 
+// -1 where the cut would build more than kMaxLevels levels (svo_b200_klt_pyramid_build refuses those).
 int level_sizes(int w, int h, int max_level, int win, int* ws, int* hs) {
   int n = 0;
-  for (int level = 0; level <= max_level && level < kMaxLevels; ++level) {
+  for (int level = 0; level <= max_level; ++level) {
+    if (level == kMaxLevels) return -1;
     ws[level] = w; hs[level] = h;
     n = level + 1;
     w = (w + 1) / 2; h = (h + 1) / 2;
@@ -98,6 +102,7 @@ int build(const uint8_t* img, int w, int h, int max_level, int win, bool deriv, 
           std::vector<std::vector<uint8_t>>* plain = nullptr, std::vector<std::vector<int16_t>>* plain_der = nullptr) {
   int ws[kMaxLevels], hs[kMaxLevels];
   const int n = level_sizes(w, h, max_level, win, ws, hs);
+  if (n < 0) return n;
   pyr.assign(n, Padded());
   std::vector<uint8_t> cur(img, img + (size_t)w * h);
   for (int l = 0; l < n; ++l) {
@@ -121,6 +126,13 @@ int build(const uint8_t* img, int w, int h, int max_level, int win, bool deriv, 
 }
 
 inline int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
+
+// floor(v) as an int (the window corner), or INT_MIN where v is NaN, +-inf or beyond int's range: the conversion is
+// undefined there in C++.  OpenCV's cvFloor gives INT_MIN for all of those on x86, and every such corner is out of bounds.
+inline int corner(float v) {
+  const float f = floorf(v);
+  return std::isfinite(f) && f >= -2147483648.f && f < 2147483648.f ? (int)f : INT_MIN;
+}
 
 // 32 strided partial sums combined pairwise (see the file header).
 struct LaneSum {
@@ -149,7 +161,8 @@ extern "C" {
 /* Exit reasons, as SVO_B200_KLT_* of include/svo_b200.h. */
 enum { KLT_CONVERGED = 0, KLT_HALF_STEP = 1, KLT_MAX_ITER = 2, KLT_OUT_OF_BOUNDS = 3, KLT_SMALL_EIG = 4, KLT_NOT_RUN = -1 };
 
-/* Level count and sizes of the LK pyramid (ws, hs: kMaxLevels ints). */
+/* Level count and sizes of the LK pyramid (ws, hs: kMaxLevels ints); -1 where OpenCV's cut would build more than
+ * kMaxLevels levels (orc_klt_pyramid and orc_klt_track return -1 there too). */
 int orc_klt_levels(int w, int h, int max_level, int win, int* ws, int* hs) { return level_sizes(w, h, max_level, win, ws, hs); }
 
 /* The levels (interior, concatenated) and, if der_out, the Scharr derivatives of each level (interleaved dx, dy). */
@@ -158,6 +171,7 @@ int orc_klt_pyramid(const uint8_t* img, int w, int h, int max_level, int win, ui
   std::vector<std::vector<uint8_t>> plain;
   std::vector<std::vector<int16_t>> plain_der;
   const int n = build(img, w, h, max_level, win, der_out != nullptr, pyr, &plain, &plain_der);
+  if (n < 0) return n;
   for (int l = 0; l < n; ++l) {
     memcpy(img_out, plain[l].data(), plain[l].size());
     img_out += plain[l].size();
@@ -171,12 +185,14 @@ int orc_klt_pyramid(const uint8_t* img, int w, int h, int max_level, int win, ui
  * level 0 ended); per point and level (kMaxLevels each, KLT_NOT_RUN / 0 / NaN where not built): level_reason, iters (steps
  * taken), and 5 margins -- min |eps^2 - delta.delta| and min |max(|sum_x|, |sum_y|) - 0.01| over the level's steps (the
  * convergence and half-step tests), minEig - 1e-4 and det - FLT_EPSILON, and the smallest distance of a tested window
- * corner to the bounds it is tested against (+inf where a test did not run).  Returns the number of levels. */
+ * corner to the bounds it is tested against (+inf where a test did not run).  Returns the number of levels (-1, and no
+ * output written, where the pyramids would need more than kMaxLevels levels). */
 int orc_klt_track(const uint8_t* prev, const uint8_t* next, int w, int h, int max_level, int win, int max_iter, double eps,
                   int n, const float* prev_pts, float* next_pts, uint8_t* status, int* reason, int* level_reason, int* iters,
                   double* margins) {
   std::vector<Padded> P, N;
   const int nl = std::min(build(prev, w, h, max_level, win, true, P), build(next, w, h, max_level, win, false, N));
+  if (nl < 0) return nl;
   const int maxL = nl - 1;
   max_iter = std::min(std::max(max_iter, 0), 100);
   eps = std::min(std::max(eps, 0.), 10.);
@@ -206,7 +222,7 @@ int orc_klt_track(const uint8_t* prev, const uint8_t* next, int w, int h, int ma
       else { nx = next_pts[2 * i] * 2.f; ny = next_pts[2 * i + 1] * 2.f; }
       next_pts[2 * i] = nx; next_pts[2 * i + 1] = ny;
       px -= hw; py -= hw;
-      int ipx = (int)floorf(px), ipy = (int)floorf(py);
+      int ipx = corner(px), ipy = corner(py);
       mg[4] = std::min(mg[4], fabs(bounds_margin(px, py, I.w, I.h, win)));
       if (ipx < -win || ipx >= I.w || ipy < -win || ipy >= I.h) {
         why = KLT_OUT_OF_BOUNDS;
@@ -247,7 +263,7 @@ int orc_klt_track(const uint8_t* prev, const uint8_t* next, int w, int h, int ma
       float pdx = 0.f, pdy = 0.f;
       why = KLT_MAX_ITER;
       for (int j = 0; j < max_iter; ++j) {
-        const int inx = (int)floorf(nx), iny = (int)floorf(ny);
+        const int inx = corner(nx), iny = corner(ny);
         mg[4] = std::min(mg[4], fabs(bounds_margin(nx, ny, J.w, J.h, win)));
         if (inx < -win || inx >= J.w || iny < -win || iny >= J.h) {
           why = KLT_OUT_OF_BOUNDS;

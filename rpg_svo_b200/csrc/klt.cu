@@ -107,7 +107,11 @@ __device__ __forceinline__ void weights(float a, float b, int& w00, int& w01, in
   w10 = __float2int_rn((1.f - a) * b * (float)(1 << 14));
   w11 = (1 << 14) - w00 - w01 - w10;
 }
-__device__ __forceinline__ bool out_of_bounds(int ix, int iy, int w, int h) { return ix < -kWin || ix >= w || iy < -kWin || iy >= h; }
+// The window corner (ix, iy) = floor of (x, y), converted with cvt.rzi, which saturates +-inf and values beyond int's range
+// (those fail the bounds) but turns NaN into 0.  OpenCV's cvFloor gives INT_MIN for NaN, so a NaN corner is out of bounds.
+__device__ __forceinline__ bool out_of_bounds(float x, float y, int ix, int iy, int w, int h) {
+  return ix < -kWin || ix >= w || iy < -kWin || iy >= h || isnan(x) || isnan(y);
+}
 
 __global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(KltLevels L, int max_iter, double eps2, int n,
                                                                const float2* __restrict__ prev_pts, float2* __restrict__ next_pts,
@@ -137,7 +141,7 @@ __global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(KltLevels L, int
     nxt = make_float2(nx, ny);
     px -= hw; py -= hw;
     const int ipx = (int)floorf(px), ipy = (int)floorf(py);
-    if (out_of_bounds(ipx, ipy, w, h)) {
+    if (out_of_bounds(px, py, ipx, ipy, w, h)) {
       e.level_reason[level] = SVO_B200_KLT_OUT_OF_BOUNDS;
       if (level == 0) st = false;
       continue;
@@ -180,7 +184,7 @@ __global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(KltLevels L, int
     int why = SVO_B200_KLT_MAX_ITER;
     for (int j = 0; j < max_iter; ++j) {
       const int inx = (int)floorf(nx), iny = (int)floorf(ny);
-      if (out_of_bounds(inx, iny, w, h)) {
+      if (out_of_bounds(nx, ny, inx, iny, w, h)) {
         why = SVO_B200_KLT_OUT_OF_BOUNDS;
         if (level == 0) st = false;
         break;
@@ -252,7 +256,10 @@ extern "C" int svo_b200_klt_pyramid_build(svo_b200_ctx* ctx, svo_b200_klt_pyrami
   if (!ctx || !pyr || !frame || max_level < 0 || (with_derivatives != 0 && with_derivatives != 1))
     return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: bad arguments");
   int w[SVO_B200_MAX_LEVELS], h[SVO_B200_MAX_LEVELS], n = 0;
-  for (int level = 0, cw = frame->width, ch = frame->height; level <= max_level && level < SVO_B200_MAX_LEVELS; ++level) {
+  for (int level = 0, cw = frame->width, ch = frame->height; level <= max_level; ++level) {
+    if (level == SVO_B200_MAX_LEVELS)  // OpenCV would build another level: refuse rather than track from a finer start
+      return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: %dx%d at max_level %d needs more than %d levels", frame->width,
+                     frame->height, max_level, SVO_B200_MAX_LEVELS);
     w[level] = cw; h[level] = ch;  // buildOpticalFlowPyramid's level cut
     n = level + 1;
     cw = (cw + 1) / 2; ch = (ch + 1) / 2;
