@@ -1413,7 +1413,9 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         }
       }
       if constexpr (!UP) pair_sync<CS>();  // barrier A: every warp's partial sums are in place
-      const int nw_pair = nwarps * CS;
+      // warps of the pair as a constant (the host launches exactly MAXT threads): the totals' loops below run one or two
+      // steps per lane, and unrolled from a constant they leave the serial path without their loop control and remainders
+      constexpr int nw_pair = G::NWC * CS;
       double tot[7];
       int n_in = 0, n_out = 0, done = 0;
       auto compute_totals = [&]() {
