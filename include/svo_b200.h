@@ -14,6 +14,7 @@
  *   svo_b200_find_epipolar_match_direct <- Matcher::findEpipolarMatchDirect   svo/include/svo/matcher.h:114-121
  *   svo_b200_depth_filter_update    <- DepthFilter::updateSeeds               svo/include/svo/depth_filter.h:155
  *                                      (Matcher::findEpipolarMatchDirect, updateSeed, computeTau inside)
+ *   (_streams: S streams' calls of reprojectMap / updateSeeds in one launch each)
  *   svo_b200_frame_*                <- svo::Frame image pyramid               svo/include/svo/frame.h:52, svo/src/frame.cpp:156-165
  *   svo_b200_klt_*                  <- initialization::trackKlt's             svo/src/initialization.cpp:127-169
  *                                      cv::calcOpticalFlowPyrLK
@@ -389,6 +390,36 @@ int svo_b200_reproject_map(svo_b200_ctx* ctx, const svo_b200_map_view* map, cons
                            int64_t* overlap_count_out, int* new_point_out, double* new_px_out, int* new_level_out,
                            int* new_type_out, double* new_grad_out, svo_b200_reproject_stats* stats);
 
+/* The arguments of one svo_b200_reproject_map call, for svo_b200_reproject_map_streams. */
+typedef struct svo_b200_reproject_stream {
+  const svo_b200_map_view* map;
+  const svo_b200_frame* const* kf_frames;
+  const svo_b200_frame* cur;
+  const double* cur_T_f_w;
+  const svo_b200_camera* cam;
+  const svo_b200_reproject_options* opt;
+  const int* cell_order;
+  int* pt_type_io;
+  int* pt_n_failed_io;
+  int* pt_n_succeeded_io;
+  uint8_t* pt_action_out;
+  int* overlap_kf_out;
+  int64_t* overlap_count_out;
+  int* new_point_out;
+  double* new_px_out;
+  int* new_level_out;
+  int* new_type_out;
+  double* new_grad_out;
+  svo_b200_reproject_stats* stats;
+} svo_b200_reproject_stream;
+/* S streams' Reprojector::reprojectMap: one device launch over the enumerated points of every stream, then each
+ * stream's one-match-per-cell replay into its own outputs.  Every output and the stats equal S calls of
+ * svo_b200_reproject_map, bit for bit.  Streams may share frame handles and map views; the _io / _out arrays of
+ * different streams must not overlap.  Every stream's arguments are checked before anything is launched or written
+ * (SVO_B200_EINVAL for S < 0, a NULL frame, an index out of range in a map view, ...), so a refused call leaves every
+ * output untouched.  S == 0 returns 0; streams that enumerate no point take no part in the launch. */
+int svo_b200_reproject_map_streams(svo_b200_ctx* ctx, int S, const svo_b200_reproject_stream* streams);
+
 /* ------------------------------------------------------------------ FAST detector ("next" row f4) -------- */
 typedef struct svo_b200_detect_options {
   int cell_size;               /* Config::gridSize() (config.cpp:32: 30) */
@@ -434,6 +465,26 @@ int svo_b200_depth_filter_update(svo_b200_ctx* ctx, const svo_b200_frame* const*
                                  int batch_counter, float* a, float* b, float* mu, float* z_range,
                                  float* sigma2, uint8_t* status_out, double* px_cur_out,
                                  double* z_out, int* n_zmssd_out);
+
+/* S streams' DepthFilter::updateSeeds in one launch; the result is bit-identical to S calls of
+ * svo_b200_depth_filter_update.  Stream s has current frame cur[s], pose cur_T_f_w[12*s .. 12*s+11], camera cam[s]
+ * (the models may differ between streams) and Seed::batch_counter batch_counter[s], and owns seeds
+ * [seed_offset[s], seed_offset[s+1]) of the per-seed arrays, which are laid out as in svo_b200_depth_filter_update
+ * (seed_offset has S+1 entries, seed_offset[0] == 0).  ref_index indexes ONE keyframe table (ref_frames, ref_T_f_w,
+ * n_ref) shared by all streams; streams may share keyframe and current-frame handles.  One options struct for all.
+ * SVO_B200_EINVAL for S < 0, a NULL frame, seed offsets that do not start at 0 or are not monotone, a ref_index or
+ * ftr_level out of range, or a max_search_level beyond a current frame's pyramid -- all checked before anything is
+ * launched or written, so a refused call leaves every output untouched.  S == 0, or no seeds at all, returns 0 without
+ * a launch (the keyframe table is then not read). */
+int svo_b200_depth_filter_update_streams(svo_b200_ctx* ctx, int S, const svo_b200_frame* const* cur /*S*/,
+                                         const double* cur_T_f_w /*S*12*/, const svo_b200_camera* cam /*S*/,
+                                         const int* batch_counter /*S*/, const int* seed_offset /*S+1*/,
+                                         const svo_b200_frame* const* ref_frames, const double* ref_T_f_w, int n_ref,
+                                         const svo_b200_depth_options* opt, const int* ref_index, const double* ftr_px,
+                                         const double* ftr_f, const int* ftr_level, const int* ftr_type,
+                                         const double* ftr_grad, const int* batch_id, float* a, float* b, float* mu,
+                                         float* z_range, float* sigma2, uint8_t* status_out, double* px_cur_out,
+                                         double* z_out, int* n_zmssd_out);
 
 /* M independent Matcher::findEpipolarMatchDirect calls (svo/include/svo/matcher.h:114-121, svo/src/matcher.cpp:179-321):
  * candidate m is reference feature (ref_index, px, f, level, type, grad) searched in `cur` along the epipolar segment of

@@ -27,7 +27,7 @@ def _nvcc() -> str:
 
 def build(force: bool = False, verbose: bool = False) -> str:
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, h) for h in os.listdir(CSRC) if h.endswith((".h", ".cuh"))]
+    deps = srcs + [os.path.join(CSRC, h) for h in os.listdir(CSRC) if h.endswith((".h", ".cuh", ".inc"))]
     deps.append(os.path.join(HERE, "..", "include", "svo_b200.h"))
     if not force and os.path.exists(OUT) and all(os.path.getmtime(d) <= os.path.getmtime(OUT) for d in deps):
         return OUT

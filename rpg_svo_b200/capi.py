@@ -526,6 +526,49 @@ def _find_epipolar_match_direct(self, ref_frames, ref_T_f_w, cur: Frame, cur_T_f
                 reject=rej[:M].astype(bool), A_cur_ref=A[:M].reshape(M, 2, 2), n_zmssd=nz[:M])
 
 
+def _depth_filter_update_streams(self, streams, ref_frames, ref_T_f_w, max_n_kfs=3, sigma2_thresh=200.0, max_search_level=2,
+                                 align_max_iter=10, max_epi_search_steps=1000):
+    """S streams' DepthFilter::updateSeeds in one launch (svo_b200_depth_filter_update_streams).  `streams`: one dict per
+    stream with cur (Frame), cur_T_f_w, cam, batch_counter and the per-seed arrays of depth_filter_update (ref_index,
+    ftr_px, ftr_f, ftr_level, ftr_type, ftr_grad, batch_id, seeds); ref_index indexes the shared keyframe table
+    ref_frames / ref_T_f_w.  Returns one dict per stream, as depth_filter_update returns."""
+    S = len(streams)
+    n = [len(s["ref_index"]) for s in streams]
+    off = np.zeros(S + 1, np.int32)
+    off[1:] = np.cumsum(n)
+    M = int(off[-1])
+
+    def cat(key, dtype):
+        parts = [np.asarray(s[key], dtype).reshape(-1) for s in streams]
+        return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, dtype), dtype)
+
+    seeds = {k: np.ascontiguousarray(np.concatenate([np.asarray(s["seeds"][k], np.float32).reshape(-1) for s in streams])
+                                     if S else np.zeros(0, np.float32), np.float32) for k in ("a", "b", "mu", "z_range", "sigma2")}
+    ri, fl, ft, bi = cat("ref_index", np.int32), cat("ftr_level", np.int32), cat("ftr_type", np.int32), cat("batch_id", np.int32)
+    fpx, ff, fg = cat("ftr_px", np.float64), cat("ftr_f", np.float64), cat("ftr_grad", np.float64)
+    status = np.zeros(max(M, 1), np.uint8)
+    pxc, z, nz = np.zeros((max(M, 1), 2)), np.zeros(max(M, 1)), np.zeros(max(M, 1), np.int32)
+    curs = (C.c_void_p * max(S, 1))(*[s["cur"].h.value for s in streams])
+    cT = c64(np.stack([np.asarray(s["cur_T_f_w"], np.float64).reshape(12) for s in streams]) if S else np.zeros((1, 12)))
+    cams = (Camera * max(S, 1))(*[cam_struct(s["cam"]) for s in streams])
+    bc = _i32([int(s["batch_counter"]) for s in streams] or [0])
+    ra = _frame_array(ref_frames)
+    refT = c64(np.asarray(ref_T_f_w, np.float64).reshape(-1) if len(ref_frames) else np.zeros(12))
+    opt = DepthOptions(max_n_kfs, sigma2_thresh, max_search_level, align_max_iter, max_epi_search_steps)
+    self._check(self.lib.svo_b200_depth_filter_update_streams(
+        self.h, S, curs, _p(cT), cams, _p(bc), _p(off), ra, _p(refT), len(ref_frames), C.byref(opt), _p(ri), _p(fpx), _p(ff),
+        _p(fl), _p(ft), _p(fg), _p(bi), _p(seeds["a"]), _p(seeds["b"]), _p(seeds["mu"]), _p(seeds["z_range"]),
+        _p(seeds["sigma2"]), _p(status), _p(pxc), _p(z), _p(nz)))
+    res = []
+    for s in range(S):
+        a, b = off[s], off[s + 1]
+        o = {k: seeds[k][a:b] for k in seeds}
+        o.update(status=status[a:b], px_cur=pxc[a:b], z=z[a:b], n_zmssd=nz[a:b])
+        res.append(o)
+    return res
+
+
+Context.depth_filter_update_streams = _depth_filter_update_streams
 Context.find_epipolar_match_direct = _find_epipolar_match_direct
 Context.align2d_batch = _align2d_batch
 Context.align1d_batch = _align1d_batch
@@ -573,10 +616,9 @@ _MV_DTYPES = dict(kf_T_f_w=np.float64, kf_keypt_pos=np.float64, kf_keypt_valid=n
                   pt_obs=np.int32, cand_point=np.int32)
 
 
-def _reproject_map(self, view: dict, kf_frames, cur: Frame, cur_T_f_w, cam, options: dict, cell_order, pt_type, pt_n_failed,
-                   pt_n_succeeded):
-    """Reprojector::reprojectMap: `view` holds the svo_b200_map_view arrays by field name.  Returns the features the
-    reference would add to the frame (new_*), the updated point state, per-point actions and the overlap keyframes."""
+def _reproject_prepare(view: dict, kf_frames, cur: Frame, cur_T_f_w, cam, options: dict, cell_order, pt_type, pt_n_failed,
+                       pt_n_succeeded):
+    """The svo_b200_reproject_stream of one call, its output arrays and the objects the call keeps alive."""
     mv, keep = MapView(), []
     for k, v in view.items():
         if k in _MV_DTYPES:
@@ -595,11 +637,18 @@ def _reproject_map(self, view: dict, kf_frames, cur: Frame, cur_T_f_w, cam, opti
     fr = _frame_array(kf_frames)
     cs = cam_struct(cam)
     co = _i32(cell_order)
-    self._check(self.lib.svo_b200_reproject_map(self.h, C.byref(mv), fr, cur.h, _p(c64(cur_T_f_w).reshape(12)), C.byref(cs),
-                                                C.byref(opt), _p(co), _p(o["pt_type"]), _p(o["pt_n_failed"]),
-                                                _p(o["pt_n_succeeded"]), _p(o["pt_action"]), _p(o["overlap_kf"]),
-                                                _p(o["overlap_count"]), _p(o["new_point"]), _p(o["new_px"]),
-                                                _p(o["new_level"]), _p(o["new_type"]), _p(o["new_grad"]), C.byref(st)))
+    cT = c64(cur_T_f_w).reshape(12)
+    keep += [mv, opt, st, fr, cs, co, cT]
+    rs = ReprojectStream(C.cast(C.pointer(mv), C.c_void_p), C.cast(fr, C.c_void_p), cur.h.value, cT.ctypes.data,
+                         C.cast(C.pointer(cs), C.c_void_p), C.cast(C.pointer(opt), C.c_void_p), co.ctypes.data,
+                         *[o[k].ctypes.data for k in ("pt_type", "pt_n_failed", "pt_n_succeeded", "pt_action", "overlap_kf",
+                                                      "overlap_count", "new_point", "new_px", "new_level", "new_type",
+                                                      "new_grad")],
+                         C.cast(C.pointer(st), C.c_void_p))
+    return rs, o, st, keep
+
+
+def _reproject_result(o: dict, st: ReprojectStats) -> dict:
     n, k = st.n_new, st.n_overlap
     for key in ("new_point", "new_px", "new_level", "new_type", "new_grad"):
         o[key] = o[key][:n]
@@ -609,6 +658,34 @@ def _reproject_map(self, view: dict, kf_frames, cur: Frame, cur_T_f_w, cam, opti
     return o
 
 
+class ReprojectStream(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("map", "kf_frames", "cur", "cur_T_f_w", "cam", "opt", "cell_order", "pt_type_io",
+                                          "pt_n_failed_io", "pt_n_succeeded_io", "pt_action_out", "overlap_kf_out",
+                                          "overlap_count_out", "new_point_out", "new_px_out", "new_level_out",
+                                          "new_type_out", "new_grad_out", "stats")]
+
+
+def _reproject_map(self, view: dict, kf_frames, cur: Frame, cur_T_f_w, cam, options: dict, cell_order, pt_type, pt_n_failed,
+                   pt_n_succeeded):
+    """Reprojector::reprojectMap: `view` holds the svo_b200_map_view arrays by field name.  Returns the features the
+    reference would add to the frame (new_*), the updated point state, per-point actions and the overlap keyframes."""
+    rs, o, st, keep = _reproject_prepare(view, kf_frames, cur, cur_T_f_w, cam, options, cell_order, pt_type, pt_n_failed,
+                                         pt_n_succeeded)
+    self._check(self.lib.svo_b200_reproject_map(self.h, *[C.c_void_p(getattr(rs, f)) for f, _ in ReprojectStream._fields_]))
+    return _reproject_result(o, st)
+
+
+def _reproject_map_streams(self, streams):
+    """S streams' Reprojector::reprojectMap with one device launch (svo_b200_reproject_map_streams).  `streams`: one dict
+    per stream with the arguments of reproject_map by name (view, kf_frames, cur, cur_T_f_w, cam, options, cell_order,
+    pt_type, pt_n_failed, pt_n_succeeded).  Returns one dict per stream, as reproject_map returns."""
+    prep = [_reproject_prepare(**s) for s in streams]
+    arr = (ReprojectStream * max(len(prep), 1))(*[p[0] for p in prep])
+    self._check(self.lib.svo_b200_reproject_map_streams(self.h, len(prep), arr))
+    return [_reproject_result(o, st) for _, o, st, _ in prep]
+
+
+Context.reproject_map_streams = _reproject_map_streams
 Context.reproject_map = _reproject_map
 
 

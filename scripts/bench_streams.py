@@ -1,0 +1,133 @@
+"""S single-stream calls against one multi-stream call of the depth filter and the reprojector, on one GPU.
+
+Depth filter: C2-like streams (752x480, 2000 seeds each, one keyframe per stream).  Reprojector: the map of bench.py's
+reprojector row (synth.make_map_case(4001, n_kfs=10, n_points=1200, n_candidates=150)) per stream; the streams cycle through
+four maps of that shape (seeds 4001..4004).  For S = 1, 8, 32, 132 it times,
+with CUDA events on the context's stream around the whole host call (staging, launch(es), copies back and, for the
+reprojector, the host replay), S back-to-back single calls and one batched call, alternating them; it reports the medians
+of --reps runs after --warmup runs of each, the kernel-only time of the batched launch (svo_b200_last_kernel_ms), and
+checks that both produce the same bits.  Prints one JSON line per (stage, S) and the card it ran on.
+
+    python scripts/bench_streams.py [--reps 50] [--warmup 5] [--streams 1,8,32,132]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from rpg_svo_b200 import capi, synth  # noqa: E402
+
+
+def card() -> dict:
+    q = "name,power.limit,clocks.sm,clocks.max.sm,clocks_throttle_reasons.active"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                             timeout=30).stdout.strip().splitlines()[0]
+        return dict(zip(q.split(","), [x.strip() for x in out.split(",")]))
+    except Exception as e:  # the measurement still stands; the card is then unknown
+        return {"error": str(e)}
+
+
+def timed(ctx, fn) -> float:
+    import torch
+
+    s = torch.cuda.ExternalStream(ctx.stream)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(s)
+    out = fn()
+    e1.record(s)
+    e1.synchronize()
+    return e0.elapsed_time(e1), out
+
+
+def bench(ctx, name, single, batched, same, reps, warmup, S):
+    for _ in range(warmup):
+        single(); batched()
+    ts, tb, tk = [], [], []
+    for _ in range(reps):
+        t, a = timed(ctx, single)
+        ts.append(t)
+        t, b = timed(ctx, batched)
+        tb.append(t)
+        tk.append(ctx.last_kernel_ms())
+    assert same(a, b), f"{name} S={S}: batched results differ from single calls"
+    r = dict(stage=name, S=S, single_calls_ms=float(np.median(ts)), batched_ms=float(np.median(tb)),
+             batched_kernel_ms=float(np.median(tk)), speedup=float(np.median(ts) / np.median(tb)), reps=reps)
+    print(json.dumps(r), flush=True)
+    return r
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--streams", default="1,8,32,132")
+    ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    a = ap.parse_args()
+    Ss = [int(x) for x in a.streams.split(",")]
+    ctx = capi.Context(0)
+    info = card()
+    print(json.dumps(dict(card=info)), flush=True)
+    results = [dict(card=info)]
+
+    # ---- depth filter: C2-like streams ----
+    scenes = [synth.make_depth_case(500 + k) for k in range(4)]
+    frames = [(ctx.frame(c["ref_pyr"]), ctx.frame(c["cur_pyr"])) for c in scenes]
+    for S in Ss:
+        sc = [scenes[s % 4] for s in range(S)]
+        fr = [frames[s % 4] for s in range(S)]
+        keys = ("ftr_px", "ftr_f", "ftr_level", "ftr_type", "ftr_grad", "batch_id")
+
+        def single(sc=sc, fr=fr):
+            return [ctx.depth_filter_update([f[0]], [c["T_ref_w"]], f[1], c["T_cur_w"], c["cam"], c["ref_index"],
+                                            *[c[k] for k in keys], c["batch_counter"], c["seeds"]) for c, f in zip(sc, fr)]
+
+        streams = [dict(cur=f[1], cur_T_f_w=c["T_cur_w"], cam=c["cam"], batch_counter=c["batch_counter"],
+                        ref_index=np.full(c["M"], s % 4, np.int32), seeds=c["seeds"], **{k: c[k] for k in keys})
+                   for s, (c, f) in enumerate(zip(sc, fr))]
+
+        def batched(streams=streams):
+            return ctx.depth_filter_update_streams(streams, [f[0] for f in frames], [c["T_ref_w"] for c in scenes])
+
+        def same(x, y):
+            return all(np.ascontiguousarray(p[k]).tobytes() == np.ascontiguousarray(q[k]).tobytes()
+                       for p, q in zip(x, y) for k in ("a", "b", "mu", "sigma2", "status", "px_cur", "z", "n_zmssd"))
+
+        results.append(bench(ctx, "depth_filter", single, batched, same, a.reps, a.warmup, S))
+
+    # ---- reprojector: bench.py's map per stream ----
+    maps = [synth.make_map_case(4001 + k, n_kfs=10, n_points=1200, n_candidates=150) for k in range(4)]
+    mfr = [([ctx.frame(p) for p in m["kf_pyr"]], ctx.frame(m["cur_pyr"])) for m in maps]
+    for S in Ss:
+        args = [dict(view=maps[s % 4]["view"], kf_frames=mfr[s % 4][0], cur=mfr[s % 4][1], cur_T_f_w=maps[s % 4]["cur_T_f_w"],
+                     cam=maps[s % 4]["cam"], options=maps[s % 4]["options"], cell_order=maps[s % 4]["cell_order"],
+                     pt_type=maps[s % 4]["pt_type"], pt_n_failed=maps[s % 4]["pt_n_failed"],
+                     pt_n_succeeded=maps[s % 4]["pt_n_succeeded"]) for s in range(S)]
+
+        def single(args=args):
+            return [ctx.reproject_map(**x) for x in args]
+
+        def batched(args=args):
+            return ctx.reproject_map_streams(args)
+
+        def same(x, y):
+            return all((np.ascontiguousarray(p[k]).tobytes() == np.ascontiguousarray(q[k]).tobytes())
+                       if isinstance(p[k], np.ndarray) else p[k] == q[k] for p, q in zip(x, y) for k in p)
+
+        results.append(bench(ctx, "reprojector", single, batched, same, a.reps, a.warmup, S))
+    if a.out:
+        with open(a.out, "w") as f:
+            for r in results:
+                f.write(json.dumps(r) + "\n")
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
