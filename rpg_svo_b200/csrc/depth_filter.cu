@@ -22,12 +22,18 @@ namespace svo {
 
 constexpr int kDfWarps = 4;
 
+// What differs between the streams of one launch, in a per-launch device table: the current frame, its pose, the camera
+// and Seed::batch_counter.
+struct DepthStream {
+  FrameDesc cur;
+  Cam cam;
+  double cur_T_f_w[12];
+  int batch_counter;
+};
+
 struct DepthParams {
   const FrameDesc* ref_frames;
   const double* ref_T_f_w;
-  FrameDesc cur;
-  double cur_T_f_w[12];
-  Cam cam;
   int M;
   const int* ref_index;
   const double* ftr_px;
@@ -36,7 +42,7 @@ struct DepthParams {
   const int* ftr_type;
   const double* ftr_grad;
   const int* batch_id;
-  int batch_counter, max_n_kfs;
+  int max_n_kfs;
   double sigma2_thresh;
   int max_search_level, align_max_iter, max_epi_search_steps;
   float *a, *b, *mu, *z_range, *sigma2;
@@ -128,58 +134,202 @@ __device__ inline double compute_tau(const Pose& T_ref_cur, const double* f, dou
   return z_plus - z;
 }
 
-__global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const DepthParams P) {  // <= 128 registers: the 500 CTAs of C2 (2000 seeds) are resident at once
-#define DF_CUR P.cur
-#define DF_CUR_T_F_W P.cur_T_f_w
-#define DF_CAM P.cam
-#define DF_BATCH_COUNTER P.batch_counter
-#define DF_STREAM_LOOKUP
-#include "depth_filter_seed.inc"
-#undef DF_CUR
-#undef DF_CUR_T_F_W
-#undef DF_CAM
-#undef DF_BATCH_COUNTER
-#undef DF_STREAM_LOOKUP
-}
+// One warp per seed of n_streams streams' concatenated seeds.  Seed i belongs to stream stream_of(seed_offset, .., i)
+// and reads that stream's current frame, pose, camera and batch counter from `streams`; `ref_index` points into one
+// keyframe table shared by all streams.  The pose products (T_ref_cur, T_cur_ref) are formed per warp: a per-stream table
+// built on the host would round differently from the device's code, and one built on the device would cost a second
+// launch.  <= 128 registers: the 500 CTAs of C2 (2000 seeds) are resident at once.
+__global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const DepthParams P,
+                                                                         const DepthStream* __restrict__ streams,
+                                                                         const int* __restrict__ seed_offset, int n_streams) {
+  __shared__ WarpAlignScratch scratch[kDfWarps];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * kDfWarps + warp;
+  if (i >= P.M) return;
+  WarpAlignScratch& S = scratch[warp];
+  for (int k = lane; k < 112; k += 32) S.pwb[k] = 0;
+  __syncwarp();
 
-// One stream of svo_b200_depth_filter_update_streams: what the single-stream call passes by value in DepthParams, read
-// from a per-launch device table instead.
-struct DepthStream {
-  FrameDesc cur;
-  Cam cam;
-  double cur_T_f_w[12];
-  int batch_counter;
-};
+  int status = 0, n_zm = 0;
+  double out_pu = 0, out_pv = 0, out_z = 0;
+  float sa = 0.f, sb = 0.f, smu = 1.f, ssig = 0.f, szr = 1.f;
+  if (!P.match_only) { sa = P.a[i]; sb = P.b[i]; smu = P.mu[i]; ssig = P.sigma2[i]; szr = P.z_range[i]; }
+  const DepthStream& st = streams[stream_of(seed_offset, n_streams, i)];
+  const Cam& cam = st.cam;
 
-// The stream that owns seed i: the last s with seed_offset[s] <= i (streams without seeds are skipped over).
-__device__ __forceinline__ int stream_of(const int* __restrict__ seed_offset, int n_streams, int i) {
-  int lo = 0, hi = n_streams - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (__ldg(seed_offset + mid) <= i) lo = mid; else hi = mid - 1;
+  do {
+    if (!P.match_only && (st.batch_counter - P.batch_id[i]) > P.max_n_kfs) { status = SVO_B200_SEED_TOO_OLD; break; }  // :216-219
+    const int r = P.ref_index[i];
+    const Pose T_ref_w = pose_from_rt12(P.ref_T_f_w + 12 * (size_t)r);
+    const Pose T_cur_w = pose_from_rt12(st.cur_T_f_w);
+    const Pose T_ref_cur = pose_mul(T_ref_w, pose_inv(T_cur_w));  // :222
+    const double fv[3] = {P.ftr_f[3 * i], P.ftr_f[3 * i + 1], P.ftr_f[3 * i + 2]};
+    float z_inv_min = 0.f;
+    double d_estimate, d_min, d_max;
+    if (!P.match_only) {
+      const double inv_mu = 1.0 / (double)smu;
+      const double p[3] = {fv[0] * inv_mu, fv[1] * inv_mu, fv[2] * inv_mu};
+      double xyz_f[3];
+      pose_apply(pose_inv(T_ref_cur), p, xyz_f);  // :223
+      if (xyz_f[2] < 0.0) { status = SVO_B200_SEED_BEHIND; break; }
+      double cu, cv;
+      world2cam(cam, xyz_f, cu, cv);
+      // isInFrame(f2c(xyz_f).cast<int>()), boundary 0; non-finite projections cannot be in frame
+      const bool fin = fabs(cu) < 1e9 && fabs(cv) < 1e9;
+      const int xi = fin ? (int)cu : -1, yi = fin ? (int)cv : -1;
+      if (!(xi >= 0 && xi < cam.width && yi >= 0 && yi < cam.height)) { status = SVO_B200_SEED_NOT_IN_FRAME; break; }
+      const float sq = sqrtf(ssig);
+      z_inv_min = __fadd_rn(smu, sq);
+      const float z_inv_max = fmaxf(__fsub_rn(smu, sq), 0.00000001f);
+      d_estimate = 1.0 / (double)smu; d_min = 1.0 / (double)z_inv_min; d_max = 1.0 / (double)z_inv_max;
+    } else {
+      d_estimate = P.d_est[i]; d_min = P.d_min[i]; d_max = P.d_max[i];
+    }
+
+    // ---------------- Matcher::findEpipolarMatchDirect (matcher.cpp:179-321) -----------------
+    bool ok = false;
+    double depth = 0.0;
+    const Pose T_cur_ref = pose_mul(T_cur_w, pose_inv(T_ref_w));  // :188
+    const int lvl = P.ftr_level[i];
+    const double pxu = P.ftr_px[2 * i], pxv = P.ftr_px[2 * i + 1];
+    double pA[3], pB[3];
+    {
+      const double a3[3] = {fv[0] * d_min, fv[1] * d_min, fv[2] * d_min};
+      const double b3[3] = {fv[0] * d_max, fv[1] * d_max, fv[2] * d_max};
+      pose_apply(T_cur_ref, a3, pA);
+      pose_apply(T_cur_ref, b3, pB);
+    }
+    const double Ax = pA[0] / pA[2], Ay = pA[1] / pA[2], Bx = pB[0] / pB[2], By = pB[1] / pB[2];  // project2d
+    const double epi_x = Ax - Bx, epi_y = Ay - By;
+    double Aff[4];
+    get_warp_matrix_affine(cam, pxu, pxv, fv, d_estimate, T_cur_ref, lvl, Aff);
+    bool reject = false;
+    int out_level = 0;
+    double out_epi_length = 0.0;
+    if (P.ftr_type[i] == 1) {  // edgelet filtering (:204-212)
+      const double gx0 = P.ftr_grad[2 * i], gy0 = P.ftr_grad[2 * i + 1];
+      const double gx = Aff[0] * gx0 + Aff[1] * gy0, gy = Aff[2] * gx0 + Aff[3] * gy0;
+      const double gn = sqrt(gx * gx + gy * gy), en = sqrt(epi_x * epi_x + epi_y * epi_y);
+      const double cosangle = fabs((gx / gn) * (epi_x / en) + (gy / gn) * (epi_y / en));
+      if (cosangle < 0.7) reject = true;
+    }
+    if (!reject) {
+      const int L = best_search_level(Aff, P.max_search_level);
+      double pAu, pAv, pBu, pBv;
+      cam_world2cam(cam, Ax, Ay, pAu, pAv);  // cam_->world2cam(A), world2cam(B)  (:217-218)
+      cam_world2cam(cam, Bx, By, pBu, pBv);
+      const double ddx = pAu - pBu, ddy = pAv - pBv;
+      const double epi_length = sqrt(ddx * ddx + ddy * ddy) / (double)(1 << L);
+      out_level = L; out_epi_length = epi_length;
+      const FrameDesc& rf = P.ref_frames[r];
+      ImgView ref_img = {rf.lvl[lvl], rf.w[lvl], rf.h[lvl]};
+      warp_warp_affine(Aff, ref_img, pxu, pxv, lvl, L, S);
+      ImgView cur_img = {st.cur.lvl[L], st.cur.w[L], st.cur.h[L]};
+      const double sc = (double)(1 << L), inv_sc = 1.0 / sc;  // a power of two: x * inv_sc == x / sc exactly
+      bool have_start = false;
+      double start_u = 0, start_v = 0;
+      if (epi_length < 2.0) {  // :226-246
+        start_u = (pAu + pBu) * 0.5;
+        start_v = (pAv + pBv) * 0.5;
+        have_start = true;
+      } else if (epi_length >= 2.0) {  // (NaN lengths fall through: the reference's size_t cast overflows -> skip)
+        const unsigned long long n0 = (unsigned long long)(epi_length / 0.7);
+        if (n0 <= (unsigned long long)P.max_epi_search_steps) {
+          const double step_x = epi_x / (double)n0, step_y = epi_y / (double)n0;
+          const double u0 = Bx - step_x, v0 = By - step_y;  // uv = B - step
+          const int n_steps = (int)n0 + 1;
+          // reference patch words + sums for the score
+          uint32_t refw[16];
+#pragma unroll
+          for (int k = 0; k < 16; ++k) refw[k] = reinterpret_cast<const uint32_t*>(S.patch)[k];
+          unsigned sA = 0, sAA = 0;
+#pragma unroll
+          for (int k = 0; k < 16; ++k) { sA = __dp4a(refw[k], 0x01010101u, sA); sAA = __dp4a(refw[k], refw[k], sAA); }
+          const int lim_x = cam.width / (1 << L) - 8, lim_y = cam.height / (1 << L) - 8;
+          long long best_key = (long long)(2000 * 64) * 4294967296LL;  // PatchScore::threshold(), strict '<'
+          for (int k = lane; k < n_steps; k += 32) {
+            // uv_k = (B - step) + k*step  (the reference accumulates uv += step; same value to ~1 ulp)
+            const double uk = fma((double)k, step_x, u0), vk = fma((double)k, step_y, v0);
+            double wu, wv;
+            cam_world2cam(cam, uk, vk, wu, wv);  // cam_->world2cam(uv)  (:272)
+            const int qx = (int)(wu * inv_sc + 0.5), qy = (int)(wv * inv_sc + 0.5);
+            int px_prev = 0, py_prev = 0;  // last_checked_pxi starts at (0,0)
+            if (k > 0) {
+              const double up = fma((double)(k - 1), step_x, u0), vp = fma((double)(k - 1), step_y, v0);
+              cam_world2cam(cam, up, vp, wu, wv);
+              px_prev = (int)(wu * inv_sc + 0.5);
+              py_prev = (int)(wv * inv_sc + 0.5);
+            }
+            if (qx == px_prev && qy == py_prev) continue;                 // :273-275
+            if (!(qx >= 8 && qx < lim_x && qy >= 8 && qy < lim_y)) continue;  // isInFrame(pxi, 8, level)
+            const int score = zmssd_score(cur_img.data, (qy - 4) * cur_img.cols + (qx - 4), cur_img.cols, refw, (int)sA, (int)sAA);
+            ++n_zm;
+            const long long key = (long long)score * 4294967296LL + (long long)k;
+            if (key < best_key && score < 2000 * 64) best_key = key;
+          }
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            const long long other = __shfl_xor_sync(0xffffffffu, best_key, o);
+            best_key = other < best_key ? other : best_key;
+            n_zm += __shfl_xor_sync(0xffffffffu, n_zm, o);
+          }
+          if (best_key < (long long)(2000 * 64) * 4294967296LL) {
+            const int kb = (int)(best_key & 0xffffffffLL);
+            const double ub = fma((double)kb, step_x, u0), vb = fma((double)kb, step_y, v0);
+            cam_world2cam(cam, ub, vb, start_u, start_v);  // px_cur_ = world2cam(uv_best)  (:299)
+            have_start = true;
+          }
+        }
+      }
+      if (have_start) {  // subpixel refinement + triangulation (:295-315 / :229-245)
+        double su = start_u / sc, sv = start_v / sc;
+        bool nan_exit = false;
+        const bool res = warp_align2d(cur_img, S, P.align_max_iter, su, sv, &nan_exit);
+        out_pu = start_u; out_pv = start_v;
+        if (res) {
+          out_pu = su * sc; out_pv = sv * sc;
+          double f_cur[3];
+          cam2world(cam, out_pu, out_pv, f_cur);
+          ok = depth_from_triangulation(T_cur_ref, fv, f_cur, depth);
+        }
+      }
+    }
+    if (P.match_only) {  // Matcher's public members after the call (matcher.h:92-101)
+      if (lane == 0) {
+        if (P.search_level_out) P.search_level_out[i] = out_level;
+        if (P.epi_length_out) P.epi_length_out[i] = out_epi_length;
+        if (P.reject_out) P.reject_out[i] = reject ? 1 : 0;
+        if (P.A_out) { P.A_out[4 * i] = Aff[0]; P.A_out[4 * i + 1] = Aff[1]; P.A_out[4 * i + 2] = Aff[2]; P.A_out[4 * i + 3] = Aff[3]; }
+      }
+      status = ok ? SVO_B200_SEED_UPDATED : SVO_B200_SEED_NO_MATCH;
+      out_z = ok ? depth : 0.0;
+      break;
+    }
+    if (!ok) {
+      sb = __fadd_rn(sb, 1.0f);  // it->b++  (:240)
+      status = SVO_B200_SEED_NO_MATCH;
+      out_pu = out_pv = 0.0;
+      break;
+    }
+    // ---------------- computeTau + updateSeed (:247-252) ---------------------------------------
+    const double px_error_angle = atan(1.0 / (2.0 * fabs(cam.fx))) * 2.0;  // :205-207
+    const double z = depth;
+    const double tau = compute_tau(T_ref_cur, fv, z, px_error_angle);
+    const double tau_inverse = 0.5 * (1.0 / fmax(0.0000001, z - tau) - 1.0 / (z + tau));
+    update_seed((float)(1. / z), (float)(tau_inverse * tau_inverse), sa, sb, smu, szr, ssig);
+    out_z = z;
+    if ((double)sqrtf(ssig) < (double)szr / P.sigma2_thresh) status = SVO_B200_SEED_CONVERGED;  // :261
+    else if (isnan(z_inv_min)) status = SVO_B200_SEED_NAN;                                       // :283
+    else status = SVO_B200_SEED_UPDATED;
+  } while (false);
+
+  if (lane == 0) {
+    if (!P.match_only) { P.a[i] = sa; P.b[i] = sb; P.mu[i] = smu; P.sigma2[i] = ssig; }
+    P.status[i] = (uint8_t)status;
+    if (P.px_cur) { P.px_cur[2 * i] = out_pu; P.px_cur[2 * i + 1] = out_pv; }
+    if (P.z) P.z[i] = out_z;
+    if (P.n_zmssd) P.n_zmssd[i] = n_zm;
   }
-  return lo;
-}
-
-// svo_b200_depth_filter_update_streams: the seeds of n_streams streams in one launch.  P holds the concatenated seed
-// arrays and the shared keyframe table, `streams` what differs per stream.  The pose products (T_ref_cur, T_cur_ref) are
-// formed per warp as in the single-stream kernel: a per-stream table built on the host would round differently from the
-// device's code, and one built on the device would cost a second launch.
-__global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_streams_kernel(const DepthParams P,
-                                                                                 const DepthStream* __restrict__ streams,
-                                                                                 const int* __restrict__ seed_offset,
-                                                                                 int n_streams) {
-#define DF_CUR st.cur
-#define DF_CUR_T_F_W st.cur_T_f_w
-#define DF_CAM st.cam
-#define DF_BATCH_COUNTER st.batch_counter
-#define DF_STREAM_LOOKUP const DepthStream& st = streams[stream_of(seed_offset, n_streams, i)];
-#include "depth_filter_seed.inc"
-#undef DF_CUR
-#undef DF_CUR_T_F_W
-#undef DF_CAM
-#undef DF_BATCH_COUNTER
-#undef DF_STREAM_LOOKUP
 }
 
 }  // namespace svo
@@ -188,61 +338,80 @@ using namespace svo;
 
 namespace {
 
-// Stages the M seeds (and, for S > 0 streams, the stream table and seed offsets), runs one depth filter launch and copies
-// the results back.  S == 0: one stream, whose frame, pose, camera and batch counter the caller has put into P.
-int depth_update_run(svo_b200_ctx* ctx, DepthParams& P, const svo_b200_frame* const* ref_frames, const double* ref_T_f_w,
-                     int n_ref, const svo_b200_frame* cur, const double* cur_T_f_w, const svo_b200_camera* cam, int S,
-                     const DepthStream* streams, const int* seed_offset, const svo_b200_depth_options* opt, int M,
-                     const int* ref_index, const double* ftr_px, const double* ftr_f, const int* ftr_level,
-                     const int* ftr_type, const double* ftr_grad, const int* batch_id, int batch_counter, float* a,
-                     float* b, float* mu, float* z_range, float* sigma2, uint8_t* status_out, double* px_cur_out,
-                     double* z_out, int* n_zmssd_out) {
+// The current frame, pose, camera and batch counter of one stream, as the kernel reads them.
+int depth_stream(svo_b200_ctx* ctx, const svo_b200_frame* cur, const double* cur_T_f_w, const svo_b200_camera* cam,
+                 int batch_counter, DepthStream& st) {
+  memset(&st, 0, sizeof(st));
+  st.cur = make_desc(cur);
+  memcpy(st.cur_T_f_w, cur_T_f_w, sizeof(double) * 12);
+  st.batch_counter = batch_counter;
+  return cam_to_dev(ctx, cam, st.cam);
+}
+
+// One depth filter launch over the M seeds of S streams, or with H.match_only over M epipolar-match candidates.  H holds
+// the caller's host arrays in the fields the kernel reads their device copies from (NULL optional outputs are not copied
+// back; with match_only, H.status receives success flags).  The arrays, the keyframe table, the stream table and the seed
+// offsets go to the device in one copy; the kernel runs once and the results come back in one copy.
+int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* const* ref_frames, const double* ref_T_f_w,
+              int n_ref, const svo_b200_depth_options* opt, const DepthStream* streams, const int* seed_offset, int S) {
+  const int M = H.M;
+  const bool mo = H.match_only != 0;
   cudaSetDevice(ctx->device);
   Carver c;
   const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),
                o_lv = c.take(sizeof(int) * M), o_ty = c.take(sizeof(int) * M), o_gr = c.take(sizeof(double) * 2 * M),
-               o_bi = c.take(sizeof(int) * M), o_rT = c.take(sizeof(double) * 12 * n_ref),
-               o_fr = c.take(sizeof(FrameDesc) * n_ref), o_zr = c.take(sizeof(float) * M);
-  const size_t o_st_tab = S ? c.take(sizeof(DepthStream) * S) : 0, o_so = S ? c.take(sizeof(int) * (S + 1)) : 0;
-  // in/out block (copied both ways)
-  const size_t o_a = c.take(sizeof(float) * M), o_b = c.take(sizeof(float) * M), o_mu = c.take(sizeof(float) * M),
-               o_s2 = c.take(sizeof(float) * M);
+               o_rT = c.take(sizeof(double) * 12 * n_ref), o_fr = c.take(sizeof(FrameDesc) * n_ref),
+               o_tab = c.take(sizeof(DepthStream) * S), o_so = c.take(sizeof(int) * (S + 1));
+  size_t o_de = 0, o_dn = 0, o_dx = 0, o_bi = 0, o_zr = 0, o_a = 0, o_b = 0, o_mu = 0, o_s2 = 0;
+  if (mo) {  // the candidates' depth ranges
+    o_de = c.take(sizeof(double) * M); o_dn = c.take(sizeof(double) * M); o_dx = c.take(sizeof(double) * M);
+  } else {   // batch ids and z_range, then the seeds (copied both ways)
+    o_bi = c.take(sizeof(int) * M); o_zr = c.take(sizeof(float) * M);
+    o_a = c.take(sizeof(float) * M); o_b = c.take(sizeof(float) * M); o_mu = c.take(sizeof(float) * M);
+    o_s2 = c.take(sizeof(float) * M);
+  }
   const size_t in_bytes = c.off;
   const size_t o_st = c.take(M), o_pc = c.take(sizeof(double) * 2 * M), o_z = c.take(sizeof(double) * M),
                o_nz = c.take(sizeof(int) * M);
+  size_t o_sl = 0, o_el = 0, o_rj = 0, o_A = 0;
+  if (mo) {  // the Matcher's scratch members
+    o_sl = c.take(sizeof(int) * M); o_el = c.take(sizeof(double) * M); o_rj = c.take(M); o_A = c.take(sizeof(double) * 4 * M);
+  }
+  const size_t o_back = mo ? o_st : o_a;
   int rc;
   if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
   if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
   uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_ri, ref_index, sizeof(int) * M);
-  memcpy(h + o_px, ftr_px, sizeof(double) * 2 * M);
-  memcpy(h + o_f, ftr_f, sizeof(double) * 3 * M);
-  memcpy(h + o_lv, ftr_level, sizeof(int) * M);
-  memcpy(h + o_ty, ftr_type, sizeof(int) * M);
-  memcpy(h + o_gr, ftr_grad, sizeof(double) * 2 * M);
-  memcpy(h + o_bi, batch_id, sizeof(int) * M);
+  memcpy(h + o_ri, H.ref_index, sizeof(int) * M);
+  memcpy(h + o_px, H.ftr_px, sizeof(double) * 2 * M);
+  memcpy(h + o_f, H.ftr_f, sizeof(double) * 3 * M);
+  memcpy(h + o_lv, H.ftr_level, sizeof(int) * M);
+  memcpy(h + o_ty, H.ftr_type, sizeof(int) * M);
+  memcpy(h + o_gr, H.ftr_grad, sizeof(double) * 2 * M);
   memcpy(h + o_rT, ref_T_f_w, sizeof(double) * 12 * n_ref);
   for (int r = 0; r < n_ref; ++r) reinterpret_cast<FrameDesc*>(h + o_fr)[r] = make_desc(ref_frames[r]);
-  memcpy(h + o_zr, z_range, sizeof(float) * M);
-  if (S) {
-    memcpy(h + o_st_tab, streams, sizeof(DepthStream) * S);
-    memcpy(h + o_so, seed_offset, sizeof(int) * (S + 1));
+  memcpy(h + o_tab, streams, sizeof(DepthStream) * S);
+  memcpy(h + o_so, seed_offset, sizeof(int) * (S + 1));
+  if (mo) {
+    memcpy(h + o_de, H.d_est, sizeof(double) * M);
+    memcpy(h + o_dn, H.d_min, sizeof(double) * M);
+    memcpy(h + o_dx, H.d_max, sizeof(double) * M);
+  } else {
+    memcpy(h + o_bi, H.batch_id, sizeof(int) * M);
+    memcpy(h + o_zr, H.z_range, sizeof(float) * M);
+    memcpy(h + o_a, H.a, sizeof(float) * M);
+    memcpy(h + o_b, H.b, sizeof(float) * M);
+    memcpy(h + o_mu, H.mu, sizeof(float) * M);
+    memcpy(h + o_s2, H.sigma2, sizeof(float) * M);
   }
-  memcpy(h + o_a, a, sizeof(float) * M);
-  memcpy(h + o_b, b, sizeof(float) * M);
-  memcpy(h + o_mu, mu, sizeof(float) * M);
-  memcpy(h + o_s2, sigma2, sizeof(float) * M);
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if (mo) SVO_CUDA_CHECK(ctx, cudaMemsetAsync(d + o_st, 0, c.off - o_st, ctx->stream));
+  DepthParams P;
+  memset(&P, 0, sizeof(P));
   P.ref_frames = reinterpret_cast<const FrameDesc*>(d + o_fr);
   P.ref_T_f_w = reinterpret_cast<const double*>(d + o_rT);
-  if (!S) {
-    P.cur = make_desc(cur);
-    memcpy(P.cur_T_f_w, cur_T_f_w, sizeof(double) * 12);
-    if ((rc = cam_to_dev(ctx, cam, P.cam))) return rc;
-    P.batch_counter = batch_counter;
-  }
   P.M = M;
   P.ref_index = reinterpret_cast<const int*>(d + o_ri);
   P.ftr_px = reinterpret_cast<const double*>(d + o_px);
@@ -250,41 +419,57 @@ int depth_update_run(svo_b200_ctx* ctx, DepthParams& P, const svo_b200_frame* co
   P.ftr_level = reinterpret_cast<const int*>(d + o_lv);
   P.ftr_type = reinterpret_cast<const int*>(d + o_ty);
   P.ftr_grad = reinterpret_cast<const double*>(d + o_gr);
-  P.batch_id = reinterpret_cast<const int*>(d + o_bi);
   P.max_n_kfs = opt->max_n_kfs;
   P.sigma2_thresh = opt->seed_convergence_sigma2_thresh;
   P.max_search_level = opt->max_search_level;
   P.align_max_iter = opt->align_max_iter;
   P.max_epi_search_steps = opt->max_epi_search_steps;
-  P.a = reinterpret_cast<float*>(d + o_a);
-  P.b = reinterpret_cast<float*>(d + o_b);
-  P.mu = reinterpret_cast<float*>(d + o_mu);
-  P.z_range = reinterpret_cast<float*>(d + o_zr);
-  P.sigma2 = reinterpret_cast<float*>(d + o_s2);
   P.status = d + o_st;
   P.px_cur = reinterpret_cast<double*>(d + o_pc);
   P.z = reinterpret_cast<double*>(d + o_z);
   P.n_zmssd = reinterpret_cast<int*>(d + o_nz);
+  P.match_only = H.match_only;
+  if (mo) {
+    P.d_est = reinterpret_cast<const double*>(d + o_de);
+    P.d_min = reinterpret_cast<const double*>(d + o_dn);
+    P.d_max = reinterpret_cast<const double*>(d + o_dx);
+    P.search_level_out = reinterpret_cast<int*>(d + o_sl);
+    P.epi_length_out = reinterpret_cast<double*>(d + o_el);
+    P.reject_out = d + o_rj;
+    P.A_out = reinterpret_cast<double*>(d + o_A);
+  } else {
+    P.batch_id = reinterpret_cast<const int*>(d + o_bi);
+    P.z_range = reinterpret_cast<float*>(d + o_zr);
+    P.a = reinterpret_cast<float*>(d + o_a);
+    P.b = reinterpret_cast<float*>(d + o_b);
+    P.mu = reinterpret_cast<float*>(d + o_mu);
+    P.sigma2 = reinterpret_cast<float*>(d + o_s2);
+  }
   const int blocks = (M + kDfWarps - 1) / kDfWarps;
   kt_begin(ctx);
-  if (S)
-    depth_filter_streams_kernel<<<blocks, kDfWarps * 32, 0, ctx->stream>>>(
-        P, reinterpret_cast<const DepthStream*>(d + o_st_tab), reinterpret_cast<const int*>(d + o_so), S);
-  else
-    depth_filter_kernel<<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P);
+  depth_filter_kernel<<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, reinterpret_cast<const DepthStream*>(d + o_tab),
+                                                                  reinterpret_cast<const int*>(d + o_so), S);
   ctx->launches++;
   kt_end(ctx);
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_a, d + o_a, c.off - o_a, cudaMemcpyDeviceToHost, ctx->stream));
+  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_back, d + o_back, c.off - o_back, cudaMemcpyDeviceToHost, ctx->stream));
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(a, h + o_a, sizeof(float) * M);
-  memcpy(b, h + o_b, sizeof(float) * M);
-  memcpy(mu, h + o_mu, sizeof(float) * M);
-  memcpy(sigma2, h + o_s2, sizeof(float) * M);
-  memcpy(status_out, h + o_st, M);
-  if (px_cur_out) memcpy(px_cur_out, h + o_pc, sizeof(double) * 2 * M);
-  if (z_out) memcpy(z_out, h + o_z, sizeof(double) * M);
-  if (n_zmssd_out) memcpy(n_zmssd_out, h + o_nz, sizeof(int) * M);
+  if (mo) {
+    for (int m = 0; m < M; ++m) H.status[m] = h[o_st + m] == SVO_B200_SEED_UPDATED;
+    if (H.search_level_out) memcpy(H.search_level_out, h + o_sl, sizeof(int) * M);
+    if (H.epi_length_out) memcpy(H.epi_length_out, h + o_el, sizeof(double) * M);
+    if (H.reject_out) memcpy(H.reject_out, h + o_rj, M);
+    if (H.A_out) memcpy(H.A_out, h + o_A, sizeof(double) * 4 * M);
+  } else {
+    memcpy(H.a, h + o_a, sizeof(float) * M);
+    memcpy(H.b, h + o_b, sizeof(float) * M);
+    memcpy(H.mu, h + o_mu, sizeof(float) * M);
+    memcpy(H.sigma2, h + o_s2, sizeof(float) * M);
+    memcpy(H.status, h + o_st, M);
+  }
+  if (H.px_cur) memcpy(H.px_cur, h + o_pc, sizeof(double) * 2 * M);
+  if (H.z) memcpy(H.z, h + o_z, sizeof(double) * M);
+  if (H.n_zmssd) memcpy(H.n_zmssd, h + o_nz, sizeof(int) * M);
   return 0;
 }
 
@@ -314,11 +499,15 @@ extern "C" int svo_b200_depth_filter_update(svo_b200_ctx* ctx, const svo_b200_fr
   if (opt->max_search_level >= cur->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: max_search_level %d >= %d pyramid levels",
                    opt->max_search_level, cur->n_levels);
-  DepthParams P;
-  memset(&P, 0, sizeof(P));
-  return depth_update_run(ctx, P, ref_frames, ref_T_f_w, n_ref, cur, cur_T_f_w, cam, 0, nullptr, nullptr, opt, M, ref_index,
-                          ftr_px, ftr_f, ftr_level, ftr_type, ftr_grad, batch_id, batch_counter, a, b, mu, z_range, sigma2,
-                          status_out, px_cur_out, z_out, n_zmssd_out);
+  DepthStream st;
+  if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, batch_counter, st)) return rc;
+  const int seed_offset[2] = {0, M};
+  DepthParams H;
+  memset(&H, 0, sizeof(H));
+  H.M = M; H.ref_index = ref_index; H.ftr_px = ftr_px; H.ftr_f = ftr_f; H.ftr_level = ftr_level; H.ftr_type = ftr_type;
+  H.ftr_grad = ftr_grad; H.batch_id = batch_id; H.a = a; H.b = b; H.mu = mu; H.z_range = z_range; H.sigma2 = sigma2;
+  H.status = status_out; H.px_cur = px_cur_out; H.z = z_out; H.n_zmssd = n_zmssd_out;
+  return depth_run(ctx, H, ref_frames, ref_T_f_w, n_ref, opt, &st, seed_offset, 1);
 }
 
 extern "C" int svo_b200_depth_filter_update_streams(svo_b200_ctx* ctx, int S, const svo_b200_frame* const* cur,
@@ -358,21 +547,15 @@ extern "C" int svo_b200_depth_filter_update_streams(svo_b200_ctx* ctx, int S, co
       return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: ftr_level[%d] outside the pyramid", m);
   }
   std::vector<DepthStream> st((size_t)S);
-  for (int s = 0; s < S; ++s) {
-    memset(&st[s], 0, sizeof(DepthStream));
-    st[s].cur = make_desc(cur[s]);
-    memcpy(st[s].cur_T_f_w, cur_T_f_w + 12 * (size_t)s, sizeof(double) * 12);
-    const int rc = cam_to_dev(ctx, cam + s, st[s].cam);
-    if (rc) return rc;
-    st[s].batch_counter = batch_counter[s];
-  }
-  DepthParams P;
-  memset(&P, 0, sizeof(P));
-  return depth_update_run(ctx, P, ref_frames, ref_T_f_w, n_ref, nullptr, nullptr, nullptr, S, st.data(), seed_offset, opt, M,
-                          ref_index, ftr_px, ftr_f, ftr_level, ftr_type, ftr_grad, batch_id, 0, a, b, mu, z_range, sigma2,
-                          status_out, px_cur_out, z_out, n_zmssd_out);
+  for (int s = 0; s < S; ++s)
+    if (const int rc = depth_stream(ctx, cur[s], cur_T_f_w + 12 * (size_t)s, cam + s, batch_counter[s], st[s])) return rc;
+  DepthParams H;
+  memset(&H, 0, sizeof(H));
+  H.M = M; H.ref_index = ref_index; H.ftr_px = ftr_px; H.ftr_f = ftr_f; H.ftr_level = ftr_level; H.ftr_type = ftr_type;
+  H.ftr_grad = ftr_grad; H.batch_id = batch_id; H.a = a; H.b = b; H.mu = mu; H.z_range = z_range; H.sigma2 = sigma2;
+  H.status = status_out; H.px_cur = px_cur_out; H.z = z_out; H.n_zmssd = n_zmssd_out;
+  return depth_run(ctx, H, ref_frames, ref_T_f_w, n_ref, opt, st.data(), seed_offset, S);
 }
-
 
 // Matcher::findEpipolarMatchDirect (svo/src/matcher.cpp:179-321) for M independent candidates: the same device code as
 // inside DepthFilter::updateSeeds, with the depth range given explicitly and the Matcher's scratch members returned.
@@ -400,79 +583,15 @@ extern "C" int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_
   if (opt->max_search_level >= cur->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: max_search_level %d >= %d pyramid levels",
                    opt->max_search_level, cur->n_levels);
-  cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),
-               o_lv = c.take(sizeof(int) * M), o_ty = c.take(sizeof(int) * M), o_gr = c.take(sizeof(double) * 2 * M),
-               o_de = c.take(sizeof(double) * M), o_dn = c.take(sizeof(double) * M), o_dx = c.take(sizeof(double) * M),
-               o_rT = c.take(sizeof(double) * 12 * n_ref), o_fr = c.take(sizeof(FrameDesc) * n_ref);
-  const size_t in_bytes = c.off;
-  const size_t o_st = c.take(M), o_pc = c.take(sizeof(double) * 2 * M), o_z = c.take(sizeof(double) * M),
-               o_nz = c.take(sizeof(int) * M), o_sl = c.take(sizeof(int) * M), o_el = c.take(sizeof(double) * M),
-               o_rj = c.take(M), o_A = c.take(sizeof(double) * 4 * M);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_ri, ref_index, sizeof(int) * M);
-  memcpy(h + o_px, ftr_px, sizeof(double) * 2 * M);
-  memcpy(h + o_f, ftr_f, sizeof(double) * 3 * M);
-  memcpy(h + o_lv, ftr_level, sizeof(int) * M);
-  memcpy(h + o_ty, ftr_type, sizeof(int) * M);
-  memcpy(h + o_gr, ftr_grad, sizeof(double) * 2 * M);
-  memcpy(h + o_de, d_estimate, sizeof(double) * M);
-  memcpy(h + o_dn, d_min, sizeof(double) * M);
-  memcpy(h + o_dx, d_max, sizeof(double) * M);
-  memcpy(h + o_rT, ref_T_f_w, sizeof(double) * 12 * n_ref);
-  for (int r = 0; r < n_ref; ++r) reinterpret_cast<FrameDesc*>(h + o_fr)[r] = make_desc(ref_frames[r]);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaMemsetAsync(d + o_st, 0, c.off - o_st, ctx->stream));
-  DepthParams P;
-  memset(&P, 0, sizeof(P));
-  P.match_only = 1;
-  P.ref_frames = reinterpret_cast<const FrameDesc*>(d + o_fr);
-  P.ref_T_f_w = reinterpret_cast<const double*>(d + o_rT);
-  P.cur = make_desc(cur);
-  memcpy(P.cur_T_f_w, cur_T_f_w, sizeof(double) * 12);
-  if ((rc = cam_to_dev(ctx, cam, P.cam))) return rc;
-  P.M = M;
-  P.ref_index = reinterpret_cast<const int*>(d + o_ri);
-  P.ftr_px = reinterpret_cast<const double*>(d + o_px);
-  P.ftr_f = reinterpret_cast<const double*>(d + o_f);
-  P.ftr_level = reinterpret_cast<const int*>(d + o_lv);
-  P.ftr_type = reinterpret_cast<const int*>(d + o_ty);
-  P.ftr_grad = reinterpret_cast<const double*>(d + o_gr);
-  P.d_est = reinterpret_cast<const double*>(d + o_de);
-  P.d_min = reinterpret_cast<const double*>(d + o_dn);
-  P.d_max = reinterpret_cast<const double*>(d + o_dx);
-  P.max_search_level = opt->max_search_level;
-  P.align_max_iter = opt->align_max_iter;
-  P.max_epi_search_steps = opt->max_epi_search_steps;
-  P.status = d + o_st;
-  P.px_cur = reinterpret_cast<double*>(d + o_pc);
-  P.z = reinterpret_cast<double*>(d + o_z);
-  P.n_zmssd = reinterpret_cast<int*>(d + o_nz);
-  P.search_level_out = reinterpret_cast<int*>(d + o_sl);
-  P.epi_length_out = reinterpret_cast<double*>(d + o_el);
-  P.reject_out = d + o_rj;
-  P.A_out = reinterpret_cast<double*>(d + o_A);
-  const int blocks = (M + kDfWarps - 1) / kDfWarps;
-  kt_begin(ctx);
-  depth_filter_kernel<<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_st, d + o_st, c.off - o_st, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int m = 0; m < M; ++m) success_out[m] = h[o_st + m] == SVO_B200_SEED_UPDATED;
-  if (depth_out) memcpy(depth_out, h + o_z, sizeof(double) * M);
-  if (px_cur_out) memcpy(px_cur_out, h + o_pc, sizeof(double) * 2 * M);
-  if (search_level_out) memcpy(search_level_out, h + o_sl, sizeof(int) * M);
-  if (epi_length_out) memcpy(epi_length_out, h + o_el, sizeof(double) * M);
-  if (reject_out) memcpy(reject_out, h + o_rj, M);
-  if (A_cur_ref_out) memcpy(A_cur_ref_out, h + o_A, sizeof(double) * 4 * M);
-  if (n_zmssd_out) memcpy(n_zmssd_out, h + o_nz, sizeof(int) * M);
-  return 0;
+  DepthStream st;
+  if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, 0, st)) return rc;
+  const int seed_offset[2] = {0, M};
+  DepthParams H;
+  memset(&H, 0, sizeof(H));
+  H.match_only = 1;
+  H.M = M; H.ref_index = ref_index; H.ftr_px = ftr_px; H.ftr_f = ftr_f; H.ftr_level = ftr_level; H.ftr_type = ftr_type;
+  H.ftr_grad = ftr_grad; H.d_est = d_estimate; H.d_min = d_min; H.d_max = d_max;
+  H.status = success_out; H.px_cur = px_cur_out; H.z = depth_out; H.n_zmssd = n_zmssd_out;
+  H.search_level_out = search_level_out; H.epi_length_out = epi_length_out; H.reject_out = reject_out; H.A_out = A_cur_ref_out;
+  return depth_run(ctx, H, ref_frames, ref_T_f_w, n_ref, opt, &st, seed_offset, 1);
 }

@@ -1,5 +1,5 @@
-// rpg_svo_b200/csrc/warp_align.cuh -- warp-cooperative device routines shared by align.cu and
-// depth_filter.cu: one warp owns one feature / seed.
+// rpg_svo_b200/csrc/warp_align.cuh -- warp-cooperative device routines shared by align.cu,
+// depth_filter.cu and reproject.cu: one warp owns one feature / seed / point.
 //
 //   warp_align2d / warp_align1d  <- feature_alignment::align2D / align1D   svo/src/feature_alignment.cpp:149-277, 30-147
 //   warp_get_warp_matrix_affine  <- warp::getWarpMatrixAffine              svo/src/matcher.cpp:33-55
@@ -31,6 +31,17 @@ static inline FrameDesc make_desc(const svo_b200_frame* f) {
   d.n_levels = f->n_levels;
   for (int l = 0; l < f->n_levels; ++l) { d.lvl[l] = f->lvl(l); d.w[l] = f->w[l]; d.h[l] = f->h[l]; }
   return d;
+}
+
+// The stream that owns item i of a launch over n_streams streams' concatenated items, stream s owning items offset[s] ..
+// offset[s + 1] - 1: the last s with offset[s] <= i (streams without items are skipped over).
+__device__ __forceinline__ int stream_of(const int* __restrict__ offset, int n_streams, int i) {
+  int lo = 0, hi = n_streams - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(offset + mid) <= i) lo = mid; else hi = mid - 1;
+  }
+  return lo;
 }
 
 

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """A/B of libsvo_b200.so builds on the flagship workload: bench.py runs once per library per round, the libraries
 alternating (SVO_B200_LIB), so that drift of the shared machine (clocks, power cap, neighbours) hits every arm alike.  Prints
-per arm the `value` runs, their median and spread, `latency_B1`, `c4_32_per_gpu`, the `e2e` values, `pose_rmse_vs_ref` and the sampled
-clocks; then runs each library once more with --dump-outputs and compares every output array bit for bit against the
+per arm the `value` runs, their median and spread, `latency_B1`, `c4_32_per_gpu`, the `e2e` values, every
+`roofline_by_kernel` row's `kernel_ms`, `pose_rmse_vs_ref` and the sampled clocks; then runs each library once more with --dump-outputs and compares every output array bit for bit against the
 first library's.
 
    python scripts/ab_bench.py --rounds 3 parent=/path/to/parent.so new=rpg_svo_b200/libsvo_b200.so [-- extra bench.py args]
@@ -59,6 +59,8 @@ def main():
                           "latency_B1_us": [round(x["latency_B1"]["device_us_per_pair"], 2) for x in r],
                           "c4_32_us": [round(x["c4_32_per_gpu"]["device_us_per_launch"], 2) for x in r],
                           "e2e": [round(x["e2e"]["value"]) if x.get("e2e") else None for x in r],
+                          "roofline_kernel_ms": {k: [round(x["roofline_by_kernel"][k]["kernel_ms"], 4) for x in r]
+                                                 for k in r[0].get("roofline_by_kernel", {})},
                           "pose_rmse_vs_ref": r[-1]["pose_rmse_vs_ref"], "clocks": [x["clocks"] for x in r]}))
     dump_args = ["--steps", "20", "--no-e2e", "--no-cpu", "--no-extras"]
     for name, lib in arms:

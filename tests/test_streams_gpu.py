@@ -2,6 +2,7 @@
 one launch each -- against S single-stream calls, bit for bit, over streams that differ in image size, camera model,
 keyframes, seed / point counts, batch counters, options and cell orders; shapes up to 257 streams; and every refusal."""
 import ctypes as C
+import dataclasses
 
 import numpy as np
 import pytest
@@ -199,7 +200,51 @@ def test_depth_streams_refusals_write_nothing(ctx):
         n0 = ctx.launch_count()
         rc, st, *_ = _raw_depth_call(ctx, **x)
         assert rc == 0 and ctx.launch_count() == n0 and np.all(st == 77)
+    # the single-stream depth filter and the epipolar matcher refuse the same way; M == 0 launches nothing
+    bad_cam = dataclasses.replace(c["cam"], model=7)
+    singles = [dict(cur=None), dict(n_ref=0), dict(ri=np.array([0, 0, 0, 0, 0, 0, 0, 1], np.int32)),
+               dict(lv=np.array([0, 0, 0, 0, 9, 0, 0, 0], np.int32)), dict(cur=small), dict(cam=bad_cam)]
+    for fn in ("update", "match"):
+        for j, over in enumerate(singles + [dict(d_min=None)] * (fn == "match") + [dict(M=0, rc=0)]):
+            x = dict(_raw_single_args(c, kf, cur, M), **over)
+            want = x.pop("rc", -1)
+            before = {k: v.copy() for k, v in x["seeds"].items()}
+            n0 = ctx.launch_count()
+            rc, outs = _raw_single_call(ctx, fn, **x)
+            assert rc == want and ctx.launch_count() == n0, (fn, j)
+            for k, o in enumerate(outs):
+                assert np.all(o == (77 if o.dtype in (np.uint8, np.int32) else 7.0)), (fn, j, k)
+            for k in before:
+                assert _same_bits(before[k], x["seeds"][k]), (fn, j, k)
     kf.destroy(); cur.destroy(); small.destroy()
+
+
+def _raw_single_args(c, kf, cur, M):
+    return dict(cur=cur, cam=c["cam"], refs=(C.c_void_p * 1)(kf.h.value), refT=c["T_ref_w"].reshape(12).copy(), n_ref=1,
+                cT=c["T_cur_w"].reshape(12).copy(), M=M, ri=np.zeros(M, np.int32), lv=np.zeros(M, np.int32), d_min=np.full(M, 0.5),
+                seeds={k: np.full(M, 0.5, np.float32) for k in ("a", "b", "mu", "z_range", "sigma2")})
+
+
+def _raw_single_call(ctx, fn, cur, cam, refs, refT, n_ref, cT, M, ri, lv, d_min, seeds):
+    """svo_b200_depth_filter_update (fn "update") or svo_b200_find_epipolar_match_direct ("match") through raw ctypes, every
+    output filled with 77 (integers) or 7.0 (doubles) beforehand; returns the return code and the outputs."""
+    opt, cs = capi.DepthOptions(3, 200.0, 2, 10, 1000), capi.cam_struct(cam)
+    n = max(M, 1)
+    px, f, g = np.zeros((n, 2)), np.tile([0.0, 0.0, 1.0], (n, 1)), np.tile([1.0, 0.0], (n, 1))
+    ty, bi, d = np.zeros(n, np.int32), np.zeros(n, np.int32), np.full(n, 1.0)
+    cur_h = cur.h if cur is not None else C.c_void_p(None)
+    head = (ctx.h, refs, capi._p(refT), n_ref, cur_h, capi._p(cT), C.byref(cs), C.byref(opt), M, capi._p(ri), capi._p(px),
+            capi._p(f), capi._p(lv), capi._p(ty), capi._p(g))
+    if fn == "update":
+        outs = [np.full(n, 77, np.uint8), np.full((n, 2), 7.0), np.full(n, 7.0), np.full(n, 77, np.int32)]
+        rc = ctx.lib.svo_b200_depth_filter_update(*head, capi._p(bi), 6, *[capi._p(seeds[k]) for k in ("a", "b", "mu", "z_range", "sigma2")],
+                                                  *[capi._p(o) for o in outs])
+    else:
+        outs = [np.full(n, 77, np.uint8), np.full(n, 7.0), np.full((n, 2), 7.0), np.full(n, 77, np.int32), np.full(n, 7.0),
+                np.full(n, 77, np.uint8), np.full((n, 4), 7.0), np.full(n, 77, np.int32)]
+        rc = ctx.lib.svo_b200_find_epipolar_match_direct(*head, capi._p(d), capi._p(d_min), capi._p(d),
+                                                         *[capi._p(o) for o in outs])
+    return rc, outs
 
 
 # ---- reprojector ---------------------------------------------------------------------------------------------------------
@@ -299,6 +344,9 @@ def test_reproject_streams_refusals_write_nothing(ctx):
     bads.append(dict(cell_order=np.full_like(cases[1]["cell_order"], -1)))
     bads.append(dict(options=dict(cases[1]["options"], max_search_level=9)))
     bads.append(dict(cur=None))
+    bads.append(dict(cam=dataclasses.replace(cases[1]["cam"], model=7)))                                    # unknown camera model
+    # a single reproject_map call refused at the camera or cell-order check has already cleared its stats and actions
+    clears_single = (False, False, True, False, False, True)
     for j, over in enumerate(bads):
         preps = []
         for i, c in enumerate(cases):
@@ -321,6 +369,16 @@ def test_reproject_streams_refusals_write_nothing(ctx):
             assert st.n_matches == 99 and st.n_trials == 99, j
             for k in o:
                 assert _same_bits(o[k], sn[k]), (j, k)
+        rs, o, st, _ = preps[1]
+        st.n_new = st.n_overlap = st.n_projected = st.n_speculative = 99
+        n0 = ctx.launch_count()
+        assert ctx.lib.svo_b200_reproject_map(ctx.h, *[C.c_void_p(getattr(rs, f)) for f, _ in capi.ReprojectStream._fields_]) == -1, j
+        assert ctx.launch_count() == n0, j
+        stats = [getattr(st, f) for f, _ in capi.ReprojectStats._fields_]
+        assert stats == ([0] * 6 if clears_single[j] else [99] * 6), (j, stats)
+        for k in o:
+            want = np.zeros_like(snap[1][k]) if k == "pt_action" and clears_single[j] else snap[1][k]   # SVO_B200_PT_NONE
+            assert _same_bits(o[k], want), (j, k)
     assert ctx.lib.svo_b200_reproject_map_streams(ctx.h, -1, None) == -1
     assert ctx.lib.svo_b200_reproject_map_streams(ctx.h, 0, None) == 0
     for f in [f for k in kfs for f in k] + curs:
