@@ -14,7 +14,7 @@
  *   svo_b200_find_epipolar_match_direct <- Matcher::findEpipolarMatchDirect   svo/include/svo/matcher.h:114-121
  *   svo_b200_depth_filter_update    <- DepthFilter::updateSeeds               svo/include/svo/depth_filter.h:155
  *                                      (Matcher::findEpipolarMatchDirect, updateSeed, computeTau inside)
- *   (_streams: S streams' calls of reprojectMap / updateSeeds in one launch each)
+ *   (_streams: S streams' calls of reprojectMap / updateSeeds / FastDetector::detect in one launch each)
  *   svo_b200_frame_*                <- svo::Frame image pyramid               svo/include/svo/frame.h:52, svo/src/frame.cpp:156-165
  *   svo_b200_klt_*                  <- initialization::trackKlt's             svo/src/initialization.cpp:127-169
  *                                      cv::calcOpticalFlowPyrLK
@@ -436,6 +436,25 @@ typedef struct svo_b200_detect_options {
 int svo_b200_fast_detect(svo_b200_ctx* ctx, const svo_b200_frame* frame, const svo_b200_detect_options* opt,
                          const uint8_t* grid_occupancy, int cap, int* x_out, int* y_out, int* level_out, float* score_out,
                          int* n_out);
+
+/* The arguments of one svo_b200_fast_detect call, for svo_b200_fast_detect_streams. */
+typedef struct svo_b200_detect_stream {
+  const svo_b200_frame* frame;
+  const svo_b200_detect_options* opt;
+  const uint8_t* grid_occupancy; /* NULL = all cells free */
+  int cap;
+  int *x_out, *y_out, *level_out;
+  float* score_out; /* may be NULL */
+  int* n_out;
+} svo_b200_detect_stream;
+/* S streams' FastDetector::detect (e.g. the keyframes of S depth filters' initializeSeeds) in one launch: one copy to the
+ * device, one launch, one copy back.  Every stream's outputs and *n_out equal one svo_b200_fast_detect call with that
+ * stream's arguments, bit for bit.  Streams may share frame handles (frame-pool frames included) with different options
+ * and grids; the output arrays of different streams must not overlap.  Every stream's arguments are checked as
+ * svo_b200_fast_detect checks them before anything is launched or written (SVO_B200_EINVAL, also for S < 0 or NULL
+ * `streams`; SVO_B200_ELIMIT when the streams' tiles exceed one launch's grid), so a refused call leaves every output
+ * untouched.  S == 0 returns 0 without a launch.  svo_b200_fast_detect is S = 1 of this call. */
+int svo_b200_fast_detect_streams(svo_b200_ctx* ctx, int S, const svo_b200_detect_stream* streams);
 
 /* ------------------------------------------------------------------ depth filter -------- */
 #define SVO_B200_SEED_TOO_OLD 1

@@ -694,21 +694,51 @@ class DetectOptions(C.Structure):
                 ("nonmax_ties_suppress", C.c_int), ("detection_threshold", C.c_double)]
 
 
+class DetectStream(C.Structure):
+    _fields_ = [("frame", C.c_void_p), ("opt", C.c_void_p), ("grid_occupancy", C.c_void_p), ("cap", C.c_int),
+                ("x_out", C.c_void_p), ("y_out", C.c_void_p), ("level_out", C.c_void_p), ("score_out", C.c_void_p),
+                ("n_out", C.c_void_p)]
+
+
+def _detect_prepare(frame: Frame, cell_size, n_pyr_levels, detection_threshold, grid_occupancy=None, fast_threshold=20,
+                    nonmax_ties_suppress=0, cap=8192):
+    """The svo_b200_detect_stream of one fast_detect call, its outputs and the objects the call keeps alive."""
+    opt = DetectOptions(int(cell_size), int(n_pyr_levels), int(fast_threshold), int(nonmax_ties_suppress), float(detection_threshold))
+    o = dict(x=np.zeros(cap, np.int32), y=np.zeros(cap, np.int32), level=np.zeros(cap, np.int32), score=np.zeros(cap, np.float32))
+    occ = None if grid_occupancy is None else _u8(grid_occupancy)
+    n = C.c_int(0)
+    ds = DetectStream(frame.h.value if frame.h else None, C.cast(C.pointer(opt), C.c_void_p), _p(occ), int(cap),
+                      *[o[k].ctypes.data for k in ("x", "y", "level", "score")], C.cast(C.pointer(n), C.c_void_p))
+    return ds, o, n, (opt, occ)
+
+
+def _detect_result(o: dict, n: C.c_int) -> dict:
+    k = min(n.value, len(o["x"]))
+    return dict(x=o["x"][:k], y=o["y"][:k], level=o["level"][:k], score=o["score"][:k], n=n.value)
+
+
 def _fast_detect(self, frame: Frame, cell_size, n_pyr_levels, detection_threshold, grid_occupancy=None, fast_threshold=20,
                  nonmax_ties_suppress=0, cap=8192):
     """FastDetector::detect: dict(x, y, level, score) of the best corner per free grid cell, cell order."""
-    opt = DetectOptions(int(cell_size), int(n_pyr_levels), int(fast_threshold), int(nonmax_ties_suppress), float(detection_threshold))
-    x, y, lv = np.zeros(cap, np.int32), np.zeros(cap, np.int32), np.zeros(cap, np.int32)
-    sc = np.zeros(cap, np.float32)
-    occ = None if grid_occupancy is None else _u8(grid_occupancy)
-    n = C.c_int(0)
-    self._check(self.lib.svo_b200_fast_detect(self.h, frame.h, C.byref(opt), _p(occ) if occ is not None else None, cap, _p(x),
-                                              _p(y), _p(lv), _p(sc), C.byref(n)))
-    k = min(n.value, cap)
-    return dict(x=x[:k], y=y[:k], level=lv[:k], score=sc[:k], n=n.value)
+    ds, o, n, _keep = _detect_prepare(frame, cell_size, n_pyr_levels, detection_threshold, grid_occupancy, fast_threshold,
+                                      nonmax_ties_suppress, cap)
+    self._check(self.lib.svo_b200_fast_detect(self.h, *[C.c_void_p(getattr(ds, f)) if f != "cap" else ds.cap
+                                                        for f, _ in DetectStream._fields_]))
+    return _detect_result(o, n)
+
+
+def _fast_detect_streams(self, streams):
+    """S streams' FastDetector::detect with one device launch (svo_b200_fast_detect_streams).  `streams`: one dict per
+    stream with the arguments of fast_detect by name (frame, cell_size, n_pyr_levels, detection_threshold and the optional
+    grid_occupancy, fast_threshold, nonmax_ties_suppress, cap).  Returns one dict per stream, as fast_detect returns."""
+    prep = [_detect_prepare(**s) for s in streams]
+    arr = (DetectStream * max(len(prep), 1))(*[p[0] for p in prep])
+    self._check(self.lib.svo_b200_fast_detect_streams(self.h, len(prep), arr))
+    return [_detect_result(o, n) for _, o, n, _ in prep]
 
 
 Context.fast_detect = _fast_detect
+Context.fast_detect_streams = _fast_detect_streams
 
 
 # ------------------------------------------------------------------ KLT tracking of the two-view initialisation

@@ -11,8 +11,8 @@
 //       + static updateSeed/computeTau stay host-side in the reference and are not re-exported
 //                                                     svo/include/svo/depth_filter.h:101-158
 //   svo::Frame / Feature / Point / Seed               svo/include/svo/{frame,feature,point,depth_filter}.h
-//   svo::streams::updateSeeds / reprojectMap          not in the reference: S objects' calls with one launch each;
-//                                                     updateSeeds is for filters without a mapper thread of their own
+//   svo::streams::updateSeeds / reprojectMap /        not in the reference: S objects' calls with one launch each;
+//     addKeyframes / detect / detectFeatures          updateSeeds / addKeyframes are for filters without a mapper thread
 // The data model is the reference's pointer graph (std::list<Feature*>, Point*); the wrappers gather it
 // into the flat arrays the C ABI takes -- that gather is the cost SURVEY.md row a18 says must be
 // counted end to end.  Differences from the reference, all forced by the missing third-party types:
@@ -543,14 +543,29 @@ class FastDetector : public AbstractDetector {
   FastDetector(int img_width, int img_height, int cell_size, int n_pyr_levels)
       : AbstractDetector(img_width, img_height, cell_size, n_pyr_levels) {}
   void detect(Frame* frame, const double detection_threshold, Features& fts, Context* ctx = nullptr) override {  // feature_detection.cpp:66-115
-    const svo_b200_detect_options opt = {cell_size_, n_pyr_levels_, 20, 0, detection_threshold};
-    const int cap = (int)grid_occupancy_.size();
-    std::vector<int> x(cap), y(cap), level(cap);
-    int n = 0;
+    Call k;
+    const svo_b200_detect_stream a = gather(frame, detection_threshold, k);
     Context& c = ctx ? *ctx : frame->context();
-    c.check(svo_b200_fast_detect(c.get(), frame->device(), &opt, grid_occupancy_.data(), cap, x.data(), y.data(), level.data(),
-                                 nullptr, &n));
-    for (int i = 0; i < n; ++i) fts.push_back(new Feature(frame, Vector2d{(double)x[i], (double)y[i]}, level[i]));
+    c.check(svo_b200_fast_detect(c.get(), a.frame, a.opt, a.grid_occupancy, a.cap, a.x_out, a.y_out, a.level_out, a.score_out,
+                                 a.n_out));
+    apply(frame, k, fts);
+  }
+
+  // The two host halves of detect around the device call, for streams::detect: the C-ABI arguments (the grid as it
+  // stands; the buffers in `k`), and the new features appended to fts with the grid reset.
+  struct Call {
+    svo_b200_detect_options opt;
+    std::vector<int> x, y, level;
+    int n = 0;
+  };
+  svo_b200_detect_stream gather(Frame* frame, double detection_threshold, Call& k) {
+    k.opt = {cell_size_, n_pyr_levels_, 20, 0, detection_threshold};
+    const int cap = (int)grid_occupancy_.size();  // at most one corner per cell
+    k.x.resize(cap); k.y.resize(cap); k.level.resize(cap);
+    return {frame->device(), &k.opt, grid_occupancy_.data(), cap, k.x.data(), k.y.data(), k.level.data(), nullptr, &k.n};
+  }
+  void apply(Frame* frame, const Call& k, Features& fts) {
+    for (int i = 0; i < k.n; ++i) fts.push_back(new Feature(frame, Vector2d{(double)k.x[i], (double)k.y[i]}, k.level[i]));
     resetGrid();
   }
 };
@@ -570,10 +585,8 @@ struct Config {  // the values of svo/src/config.cpp that the initialisation rea
 };
 
 namespace initialization {
-inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, std::vector<Vector3d>& f_vec) {  // :107-125
-  Features new_features;
-  feature_detection::FastDetector detector(frame->img_pyr_[0].cols, frame->img_pyr_[0].rows, Config::gridSize(), Config::nPyrLevels());
-  detector.detect(frame.get(), Config::triangMinCornerScore(), new_features);
+// the detected features as pixel and bearing vectors; the features are freed (:114-124)
+inline void takeFeatures(Features& new_features, std::vector<Point2f>& px_vec, std::vector<Vector3d>& f_vec) {
   px_vec.clear(); px_vec.reserve(new_features.size());
   f_vec.clear(); f_vec.reserve(new_features.size());
   for (Feature* ftr : new_features) {
@@ -581,6 +594,12 @@ inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, 
     f_vec.push_back(ftr->f);
     delete ftr;
   }
+}
+inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, std::vector<Vector3d>& f_vec) {  // :107-125
+  Features new_features;
+  feature_detection::FastDetector detector(frame->img_pyr_[0].cols, frame->img_pyr_[0].rows, Config::gridSize(), Config::nPyrLevels());
+  detector.detect(frame.get(), Config::triangMinCornerScore(), new_features);
+  takeFeatures(new_features, px_vec, f_vec);
 }
 
 // calcOpticalFlowPyrLK(ref, cur, px_ref, px_cur, ..., Size(30, 30), 4, (COUNT + EPS, 30, 0.001), OPTFLOW_USE_INITIAL_FLOW),
@@ -615,12 +634,61 @@ inline void trackKlt(const FramePtr& frame_ref, const FramePtr& frame_cur, std::
 }
 }  // namespace initialization
 
+// Many camera streams per GPU: S detectors' FastDetector::detect, and S frames' initialization::detectFeatures, with one
+// device launch (svo_b200_fast_detect_streams).  The device work runs on `ctx`, by default the context of frames[0];
+// every frame must live on that context's device.
+namespace streams {
+
+// FastDetector::detect(frames[s], thresholds[s], fts[s]) of every detectors[s]: fts[s] gets the features the detector's
+// own call would append, and every detector's grid is reset afterwards, as detect resets it.  A detector listed twice is
+// refused (std::invalid_argument) before anything changes.
+inline void detect(const std::vector<feature_detection::FastDetector*>& detectors, const std::vector<FramePtr>& frames,
+                   const std::vector<double>& thresholds, std::vector<Features>& fts, Context* ctx = nullptr) {
+  const size_t S = detectors.size();
+  if (frames.size() != S || thresholds.size() != S || fts.size() != S)
+    throw std::invalid_argument("streams::detect: one frame, threshold and feature list per detector");
+  if (S == 0) return;
+  for (size_t s = 0; s < S; ++s) {
+    if (!detectors[s] || !frames[s]) throw std::invalid_argument("streams::detect: NULL detector or frame");
+    for (size_t t = 0; t < s; ++t)
+      if (detectors[t] == detectors[s]) throw std::invalid_argument("streams::detect: a detector is listed twice");
+  }
+  std::vector<feature_detection::FastDetector::Call> k(S);
+  std::vector<svo_b200_detect_stream> a(S);
+  for (size_t s = 0; s < S; ++s) a[s] = detectors[s]->gather(frames[s].get(), thresholds[s], k[s]);
+  Context& c = ctx ? *ctx : frames[0]->context();
+  c.check(svo_b200_fast_detect_streams(c.get(), (int)S, a.data()));
+  for (size_t s = 0; s < S; ++s) detectors[s]->apply(frames[s].get(), k[s], fts[s]);
+}
+
+// initialization::detectFeatures(frames[s], px_vecs[s], f_vecs[s]) of every frame.
+inline void detectFeatures(const std::vector<FramePtr>& frames, std::vector<std::vector<Point2f>>& px_vecs,
+                           std::vector<std::vector<Vector3d>>& f_vecs) {
+  const size_t S = frames.size();
+  if (px_vecs.size() != S || f_vecs.size() != S) throw std::invalid_argument("streams::detectFeatures: one output pair per frame");
+  std::vector<std::unique_ptr<feature_detection::FastDetector>> owned;
+  std::vector<feature_detection::FastDetector*> detectors;
+  for (const FramePtr& frame : frames) {
+    if (!frame) throw std::invalid_argument("streams::detectFeatures: NULL frame");
+    owned.emplace_back(new feature_detection::FastDetector(frame->img_pyr_[0].cols, frame->img_pyr_[0].rows, Config::gridSize(),
+                                                           Config::nPyrLevels()));
+    detectors.push_back(owned.back().get());
+  }
+  std::vector<Features> fts(S);
+  detect(detectors, frames, std::vector<double>(S, Config::triangMinCornerScore()), fts);
+  for (size_t s = 0; s < S; ++s) initialization::takeFeatures(fts[s], px_vecs[s], f_vecs[s]);
+}
+
+}  // namespace streams
+
 class DepthFilter;
 class Reprojector;
 // Many camera streams per GPU: S objects' updateSeeds / reprojectMap with one device launch each (defined after the
 // classes, see there).
 namespace streams {
 void updateSeeds(const std::vector<DepthFilter*>& filters, const std::vector<FramePtr>& frames);
+void addKeyframes(const std::vector<DepthFilter*>& filters, const std::vector<FramePtr>& frames,
+                  const std::vector<double>& depth_mean, const std::vector<double>& depth_min);
 void reprojectMap(const std::vector<Reprojector*>& reprojectors, const std::vector<FramePtr>& frames,
                   std::vector<std::vector<std::pair<FramePtr, size_t>>>& overlap_kfs);
 }  // namespace streams
@@ -751,6 +819,8 @@ class DepthFilter {
 
  protected:
   friend void streams::updateSeeds(const std::vector<DepthFilter*>&, const std::vector<FramePtr>&);
+  friend void streams::addKeyframes(const std::vector<DepthFilter*>&, const std::vector<FramePtr>&, const std::vector<double>&,
+                                    const std::vector<double>&);
   svo_b200_depth_options abiOptions() const {
     return {options_.max_n_kfs, options_.seed_convergence_sigma2_thresh, options_.max_search_level, 10, 1000};
   }
@@ -1171,6 +1241,49 @@ inline void updateSeeds(const std::vector<DepthFilter*>& filters, const std::vec
     std::copy(px_cur.begin() + 2 * o, px_cur.begin() + 2 * (o + n), x.px_cur.begin());
     std::copy(z.begin() + o, z.begin() + o + n, x.z.begin());
     filters[s]->applySeeds(frames[s], x);
+  }
+}
+
+// DepthFilter::addKeyframe(frames[s], depth_mean[s], depth_min[s]) of every filters[s] -- initializeSeeds with one
+// detection launch -- for filters WITHOUT a thread of their own (the reference's synchronous mode, depth_filter.cpp:110-113).
+// Every filter's grid is filled from its keyframe's features, all keyframes are detected in one launch, and then each
+// filter takes its new seeds in stream order: Seed::batch_counter() and Seed::seed_counter() are process-wide, and only
+// that order leaves batch and seed ids as S sequential calls leave them.  Refused with std::invalid_argument before any
+// object changes: a filter listed twice, one with a thread, one without a detector or with one that is not a
+// FastDetector, and two filters sharing one detector (sequential calls would fill, detect and reset its grid once per
+// filter, which one launch cannot reproduce).
+inline void addKeyframes(const std::vector<DepthFilter*>& filters, const std::vector<FramePtr>& frames,
+                         const std::vector<double>& depth_mean, const std::vector<double>& depth_min) {
+  const size_t S = filters.size();
+  if (frames.size() != S || depth_mean.size() != S || depth_min.size() != S)
+    throw std::invalid_argument("streams::addKeyframes: one frame and one depth pair per filter");
+  if (S == 0) return;
+  std::vector<feature_detection::FastDetector*> detectors(S);
+  for (size_t s = 0; s < S; ++s) {
+    if (!filters[s] || !frames[s]) throw std::invalid_argument("streams::addKeyframes: NULL filter or frame");
+    if (filters[s]->thread_) throw std::invalid_argument("streams::addKeyframes: a filter runs its own mapper thread");
+    if (!filters[s]->feature_detector_) throw std::invalid_argument("streams::addKeyframes: a filter has no feature detector");
+    detectors[s] = dynamic_cast<feature_detection::FastDetector*>(filters[s]->feature_detector_.get());
+    if (!detectors[s]) throw std::invalid_argument("streams::addKeyframes: a filter's detector is not a FastDetector");
+    for (size_t t = 0; t < s; ++t) {
+      if (filters[t] == filters[s]) throw std::invalid_argument("streams::addKeyframes: a filter is listed twice");
+      if (detectors[t] == detectors[s]) throw std::invalid_argument("streams::addKeyframes: two filters share one detector");
+    }
+  }
+  std::vector<double> thresholds(S);
+  for (size_t s = 0; s < S; ++s) {  // addKeyframe (:103-104), then initializeSeeds up to the detection (:119-120)
+    DepthFilter& df = *filters[s];
+    df.new_keyframe_min_depth_ = depth_min[s];
+    df.new_keyframe_mean_depth_ = depth_mean[s];
+    df.feature_detector_->setExistingFeatures(frames[s]->fts_);
+    thresholds[s] = df.triang_min_corner_score_;
+  }
+  std::vector<Features> fts(S);
+  detect(detectors, frames, thresholds, fts, filters[0]->ctx_);
+  for (size_t s = 0; s < S; ++s) {
+    DepthFilter& df = *filters[s];
+    df.addKeyframe(frames[s], std::vector<Feature*>(fts[s].begin(), fts[s].end()), df.new_keyframe_mean_depth_,
+                   df.new_keyframe_min_depth_);
   }
 }
 

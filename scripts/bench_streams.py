@@ -1,10 +1,12 @@
-"""S single-stream calls against one multi-stream call of the depth filter and the reprojector, on one GPU.
+"""S single-stream calls against one multi-stream call of the depth filter, the reprojector and the FAST detector, on one GPU.
 
 Depth filter: C2-like streams (752x480, 2000 seeds each, one keyframe per stream).  Reprojector: the map of bench.py's
 reprojector row (synth.make_map_case(4001, n_kfs=10, n_points=1200, n_candidates=150)) per stream; the streams cycle through
-four maps of that shape (seeds 4001..4004).  For S = 1, 8, 32, 132 it times,
+four maps of that shape (seeds 4001..4004).  FAST detector: the keyframe seeding of DepthFilter::initializeSeeds, one
+752x480 keyframe with 3 pyramid levels per stream, 30-px cells, the cells of about 120 existing features occupied; the
+streams cycle through four such keyframes.  For S = 1, 8, 32, 132 it times,
 with CUDA events on the context's stream around the whole host call (staging, launch(es), copies back and, for the
-reprojector, the host replay), S back-to-back single calls and one batched call, alternating them; it reports the medians
+reprojector and the detector, the host replay or decode), S back-to-back single calls and one batched call, alternating them; it reports the medians
 of --reps runs after --warmup runs of each, the kernel-only time of the batched launch (svo_b200_last_kernel_ms), and
 checks that both produce the same bits.  Prints one JSON line per (stage, S) and the card it ran on.
 
@@ -122,6 +124,31 @@ def main():
                        if isinstance(p[k], np.ndarray) else p[k] == q[k] for p, q in zip(x, y) for k in p)
 
         results.append(bench(ctx, "reprojector", single, batched, same, a.reps, a.warmup, S))
+
+    # ---- FAST detector: keyframe seeding ----
+    kfs = []
+    for k in range(4):
+        pyr = synth.make_two_view(600 + k, n_levels=3)["ref_pyr"]
+        rng = np.random.default_rng(600 + k)
+        occ = np.zeros(26 * 16, np.uint8)                                       # ceil(752/30) x ceil(480/30) cells
+        px = rng.uniform([0, 0], [752, 480], (120, 2)).astype(int)             # the keyframe's existing features
+        occ[(px[:, 1] // 30) * 26 + px[:, 0] // 30] = 1
+        kfs.append((ctx.frame(pyr), occ))
+    for S in Ss:
+        args = [dict(frame=kfs[s % 4][0], cell_size=30, n_pyr_levels=3, detection_threshold=20.0, grid_occupancy=kfs[s % 4][1])
+                for s in range(S)]
+
+        def single(args=args):
+            return [ctx.fast_detect(**x) for x in args]
+
+        def batched(args=args):
+            return ctx.fast_detect_streams(args)
+
+        def same(x, y):
+            return all(p["n"] == q["n"] and all(p[k].tobytes() == q[k].tobytes() for k in ("x", "y", "level", "score"))
+                       for p, q in zip(x, y))
+
+        results.append(bench(ctx, "fast_detect", single, batched, same, a.reps, a.warmup, S))
     if a.out:
         with open(a.out, "w") as f:
             for r in results:
