@@ -315,7 +315,9 @@ int svo_b200_pose_optimize(svo_b200_ctx* ctx, double reproj_thresh, int n_iter,
                            svo_b200_pose_opt_result* out);
 
 /* B frames in one launch (one CTA per frame): frame b owns observations [obs_offset[b], obs_offset[b+1]) of the
- * concatenated arrays; fx[b] = that frame's cam->errorMultiplier2().  Same results as B single calls. */
+ * concatenated arrays; fx[b] = that frame's cam->errorMultiplier2().  Same results as B single calls.
+ * Requires 0 <= obs_offset[0] <= obs_offset[1] <= ... <= obs_offset[B]; otherwise SVO_B200_EINVAL, nothing written
+ * but out (zeroed). */
 int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double reproj_thresh, int n_iter, const double* fx /*B*/,
                                  double* T_f_w_io /*B*12*/, const int* obs_offset /*B+1*/, const double* f,
                                  const double* point_pos, const int* level, uint8_t* has_point_io,
@@ -324,7 +326,10 @@ int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double reproj_thresh,
 /* Point::optimize (svo/src/point.cpp:119-177) for P independent points ("next" row f3: structure
  * refinement after the pose optimizer, frame_handler_base.cpp:178-196).  Point p owns observations
  * [obs_offset[p], obs_offset[p+1]); observation o is seen from frame obs_frame[o] (pose frame_T_f_w) with
- * unit bearing obs_f[o].  pos_io: P*3 world positions, updated in place. */
+ * unit bearing obs_f[o].  pos_io: P*3 world positions, updated in place.
+ * Requires 0 <= obs_offset[0] <= obs_offset[1] <= ... <= obs_offset[P] and 0 <= obs_frame[o] < n_frames for the
+ * observations in [obs_offset[0], obs_offset[P]) (entries before obs_offset[0] are not read); otherwise
+ * SVO_B200_EINVAL before anything is launched or written. */
 int svo_b200_point_optimize_batch(svo_b200_ctx* ctx, int P, int n_iter, const int* obs_offset,
                                   const int* obs_frame, const double* obs_f, const double* frame_T_f_w,
                                   int n_frames, double* pos_io);
@@ -337,7 +342,8 @@ typedef struct svo_b200_map_view {
   const double* kf_T_f_w;        /* n_kfs*12 */
   const double* kf_keypt_pos;    /* n_kfs*5*3: key_pts_[i]->point->pos_ (frame.h:53) */
   const uint8_t* kf_keypt_valid; /* n_kfs*5: key_pts_[i] != NULL */
-  const int* kf_fts_offset;      /* n_kfs+1: Frame::fts_ of keyframe k = kf_fts[offset[k] .. offset[k+1]) */
+  const int* kf_fts_offset;      /* n_kfs+1: Frame::fts_ of keyframe k = kf_fts[offset[k] .. offset[k+1]);
+                                    0 <= offset[0] <= offset[1] <= ... <= offset[n_kfs] */
   const int* kf_fts;             /* indices into the feature table, fts_ list order */
   int n_ftrs;                    /* feature table: every Feature a Frame::fts_ or Point::obs_ entry refers to */
   const int* ftr_kf;             /* Feature::frame as keyframe index */
@@ -349,7 +355,8 @@ typedef struct svo_b200_map_view {
   const int* ftr_point;          /* Feature::point as point index, -1 = NULL */
   int n_points;
   const double* pt_pos;          /* n_points*3 */
-  const int* pt_obs_offset;      /* n_points+1 */
+  const int* pt_obs_offset;      /* n_points+1: Point::obs_ of point p = pt_obs[offset[p] .. offset[p+1]);
+                                    0 <= offset[0] <= offset[1] <= ... <= offset[n_points] */
   const int* pt_obs;             /* Point::obs_ in list order, as feature-table indices */
   int n_candidates;
   const int* cand_point;         /* MapPointCandidates::candidates_ in list order, as point indices (map.h:44) */

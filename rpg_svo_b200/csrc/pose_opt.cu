@@ -514,6 +514,7 @@ extern "C" int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double rep
   if (B == 0) return 0;
   memset(out, 0, sizeof(*out) * (size_t)B);
   const int base = obs_offset[0], total = obs_offset[B] - base;
+  if (base < 0) return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: obs_offset[0] is negative");
   int max_n = 0;
   for (int b = 0; b < B; ++b) {
     const int n = obs_offset[b + 1] - obs_offset[b];
@@ -681,6 +682,10 @@ extern "C" int svo_b200_point_optimize_batch(svo_b200_ctx* ctx, int P, int n_ite
   if (!ctx || P < 0 || n_iter < 0 || n_frames <= 0 || (P > 0 && (!obs_offset || !obs_frame || !obs_f || !frame_T_f_w || !pos_io)))
     return set_err(ctx, SVO_B200_EINVAL, "point_optimize_batch: bad arguments");
   if (P == 0) return 0;
+  // the kernel walks [off[p], off[p+1]) of the staged observations: every such range must lie inside the staged ones
+  for (int p = 0; p <= P; ++p)
+    if (obs_offset[p] < (p ? obs_offset[p - 1] : 0))
+      return set_err(ctx, SVO_B200_EINVAL, "point_optimize_batch: obs_offset[%d] is negative or decreasing", p);
   const int n_obs = obs_offset[P] - obs_offset[0];
   for (int o = 0; o < n_obs; ++o)
     if (obs_frame[obs_offset[0] + o] < 0 || obs_frame[obs_offset[0] + o] >= n_frames)

@@ -175,6 +175,14 @@ int reproject_check(svo_b200_ctx* ctx, const svo_b200_reproject_stream& a) {
     return set_err(ctx, SVO_B200_EINVAL, "reproject_map: NULL array in the map view");
   for (int k = 0; k < m->n_kfs; ++k)
     if (!kf_frames[k]) return set_err(ctx, SVO_B200_EINVAL, "reproject_map: kf_frames[%d] is NULL", k);
+  // the device and reproject_enumerate walk every [offset[i], offset[i+1]) range: each must lie inside the range
+  // [0, offset[n]) whose entries are checked below
+  for (int k = 0; k <= m->n_kfs && m->n_kfs > 0; ++k)
+    if (m->kf_fts_offset[k] < (k ? m->kf_fts_offset[k - 1] : 0))
+      return set_err(ctx, SVO_B200_EINVAL, "reproject_map: kf_fts_offset[%d] is negative or decreasing", k);
+  for (int p = 0; p <= m->n_points && m->n_points > 0; ++p)
+    if (m->pt_obs_offset[p] < (p ? m->pt_obs_offset[p - 1] : 0))
+      return set_err(ctx, SVO_B200_EINVAL, "reproject_map: pt_obs_offset[%d] is negative or decreasing", p);
   const int n_kf_fts = m->n_kfs ? m->kf_fts_offset[m->n_kfs] : 0, n_obs_total = m->n_points ? m->pt_obs_offset[m->n_points] : 0;
   if (n_kf_fts < 0 || n_obs_total < 0 || (n_kf_fts > 0 && !m->kf_fts) || (n_obs_total > 0 && !m->pt_obs))
     return set_err(ctx, SVO_B200_EINVAL, "reproject_map: inconsistent offsets in the map view");

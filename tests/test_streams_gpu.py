@@ -345,8 +345,13 @@ def test_reproject_streams_refusals_write_nothing(ctx):
     bads.append(dict(options=dict(cases[1]["options"], max_search_level=9)))
     bads.append(dict(cur=None))
     bads.append(dict(cam=dataclasses.replace(cases[1]["cam"], model=7)))                                    # unknown camera model
+    # offset tables whose last entry is in range but whose interior is not: a point's observation range reaching past
+    # pt_obs (then decreasing), and a negative first keyframe-feature offset
+    v = dict(cases[1]["view"]); v["pt_obs_offset"] = v["pt_obs_offset"].copy(); v["pt_obs_offset"][1] = v["pt_obs_offset"][-1] + 1000
+    bads.append(dict(view=v))
+    v = dict(cases[1]["view"]); v["kf_fts_offset"] = v["kf_fts_offset"].copy(); v["kf_fts_offset"][0] = -3; bads.append(dict(view=v))
     # a single reproject_map call refused at the camera or cell-order check has already cleared its stats and actions
-    clears_single = (False, False, True, False, False, True)
+    clears_single = (False, False, True, False, False, True, False, False)
     for j, over in enumerate(bads):
         preps = []
         for i, c in enumerate(cases):
