@@ -93,35 +93,11 @@ __device__ __forceinline__ uint32_t half2(uint32_t top, uint32_t bot, bool avg) 
 __device__ __forceinline__ uint32_t half1(uint32_t a, uint32_t b, uint32_t c, uint32_t d, bool avg) {  // one output pixel
   return avg ? ((((a + c + 1u) >> 1) + ((b + d + 1u) >> 1) + 1u) >> 1) : ((a + b + c + d) >> 2);
 }
-// HBM-bound byte kernel: each thread produces 4 output pixels from two 8-byte row segments (coalesced 64-bit loads,
-// one 32-bit store).  `avg` selects the SSE2 rounding.
-__global__ void half_sample_kernel(const uint8_t* __restrict__ in, int in_w, int in_h,
-                                   uint8_t* __restrict__ out, int out_w, int out_h, int avg) {
-  const int quads = (out_w + 3) / 4;
-  const int total = quads * out_h;
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-    const int y = idx / quads, qx = idx - y * quads;
-    const int x0 = qx * 4;
-    const uint8_t* top = in + (size_t)(2 * y) * in_w + 2 * x0;
-    const uint8_t* bot = top + in_w;
-    if (x0 + 4 <= out_w && ((in_w & 7) == 0)) {
-      const uint2 t = *reinterpret_cast<const uint2*>(top);
-      const uint2 b = *reinterpret_cast<const uint2*>(bot);
-      const uint32_t q0 = half2(t.x, b.x, avg != 0), q1 = half2(t.y, b.y, avg != 0);
-      const uint32_t r = (q0 & 0xffu) | ((q0 >> 8) & 0xff00u) | ((q1 & 0xffu) << 16) | ((q1 << 8) & 0xff000000u);
-      *reinterpret_cast<uint32_t*>(out + (size_t)y * out_w + x0) = r;
-    } else {
-      for (int k = 0; k < 4 && x0 + k < out_w; ++k)
-        out[(size_t)y * out_w + x0 + k] = (uint8_t)half1(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1], avg != 0);
-    }
-  }
-}
-
 
 // Fused pyramid build for a batch of frames laid out with a constant stride: one CTA turns a
 // 128x16 tile of level 0 into the matching 64x8 / 32x4 / 16x2 / 8x1 tiles of levels 1..4 (as many as
-// the frame has), reading level 0 from HBM exactly once.  Same arithmetic as half_sample_kernel
-// (level l+1 = (a+b+c+d)/4 of level l), so the result is identical to the level-by-level build.
+// the frame has), reading level 0 from HBM exactly once.  Every level is the halfSample of the one
+// above it, so a deeper pyramid is built by further passes starting from the last level built.
 // The kernel also writes the block-tiled copies (ctx.h) of the levels it reads or produces: whole 4x4 blocks from the
 // level-0 .. level-2 tiles, and the rows of level 3 / 4 blocks that fall into this tile.
 struct PyrGeom {
@@ -276,8 +252,9 @@ __global__ void __launch_bounds__(256) pyramid_l0_l1_stream_kernel(const uint8_t
 }
 
 // Block-tiled copy of levels [first_level, first_level + gridDim.y) of `count` frames, level l of frame i at lvl[l] +
-// i * stride[l], its copy at tl[l] + i * tstride[l]: one thread per 4x4 block, zero outside the level.  Tiles the levels no pyramid kernel tiles: levels
-// uploaded from the host, and levels below the fused kernel's.
+// i * stride[l], its copy at tl[l] + i * tstride[l]: one thread per 4x4 block, zero outside the level.  Tiles the levels no
+// pyramid kernel tiles: levels uploaded from the host below the first fused pass, and the streaming kernel's level 1 of a
+// two-level pyramid.
 struct TileGeom {
   uint8_t* lvl[SVO_B200_MAX_LEVELS];
   unsigned long long stride[SVO_B200_MAX_LEVELS];
@@ -312,18 +289,17 @@ __global__ void __launch_bounds__(256) tile_levels_kernel(TileGeom g, int first_
   }
 }
 
-// tile_levels_kernel over levels [from, to) of `count` frames, level l of frame i at lvl[l] + i * stride[l], its copy at
-// tl[l] + i * tstride[l] (strides: nullptr for one frame)
-static int tile_levels(svo_b200_ctx* ctx, uint8_t* const* lvl, const size_t* stride, uint8_t* const* tl, const size_t* tstride,
-                       const int* w, const int* h, int from, int to, int count) {
+// tile_levels_kernel over levels [from, to) of frames [first, first + count) of `pool`
+static int tile_levels(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int first, int count, int from, int to) {
   if (from >= to) return 0;
+  const svo_b200_frame& f = pool->frames[first];
   TileGeom g;
   memset(&g, 0, sizeof(g));
   for (int l = from; l < to; ++l) {
-    g.lvl[l] = lvl[l]; g.stride[l] = stride ? stride[l] : 0; g.tl[l] = tl[l]; g.tstride[l] = tstride ? tstride[l] : 0;
-    g.w[l] = w[l]; g.h[l] = h[l];
+    g.lvl[l] = f.lv[l]; g.stride[l] = pool->stride[l]; g.tl[l] = f.tv[l]; g.tstride[l] = pool->tstride[l];
+    g.w[l] = f.w[l]; g.h[l] = f.h[l];
   }
-  const long long n = (long long)((w[from] + 3) / 4) * ((h[from] + 3) / 4) * count;  // blocks of the largest level
+  const long long n = (long long)((f.w[from] + 3) / 4) * ((f.h[from] + 3) / 4) * count;  // blocks of the largest level
   long long blocks = (n + 255) / 256;
   if (blocks > ctx->sm_count * 8LL) blocks = ctx->sm_count * 8LL;
   tile_levels_kernel<<<dim3((unsigned)blocks, (unsigned)(to - from)), 256, 0, ctx->stream>>>(g, from, count);
@@ -338,22 +314,92 @@ static inline int pyr_avg(const svo_b200_ctx* ctx, int src_w) {
   return ctx->pyramid_rule == SVO_B200_PYR_X86 && (src_w % 16) == 0;
 }
 
-// Levels [from_level, n_levels) of one frame from the level above, then the tiled copies of levels [tile_from, n_levels).
-static int build_levels(svo_b200_ctx* ctx, svo_b200_frame* fr, int from_level, int tile_from, bool timed = true) {
-  if (timed) kt_begin(ctx);
-  for (int l = from_level; l < fr->n_levels; ++l) {
-    const int total = ((fr->w[l] + 3) / 4) * fr->h[l];
-    if (total <= 0) continue;
-    const int threads = 256;
-    int blocks = (total + threads - 1) / threads;
-    if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-    half_sample_kernel<<<blocks, threads, 0, ctx->stream>>>(fr->lvl(l - 1), fr->w[l - 1], fr->h[l - 1],
-                                                            fr->lvl(l), fr->w[l], fr->h[l], pyr_avg(ctx, fr->w[l - 1]));
+// The missing levels and the tiled copies of every level of frames [first, first + count) of `pool`, whose levels
+// [0, n_given) are on the device.  Level 0 -> 1 with the streaming kernel when only level 0 is given and the width allows
+// 128-bit rows, then passes of the fused kernel over the whole window, each from the highest level built so far to up to
+// four levels further.
+static int build_pyramid(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int first, int count, int n_given) {
+  const svo_b200_frame& f0 = pool->frames[0];
+  const int n_levels = f0.n_levels;
+  kt_begin(ctx);
+  int top = n_given - 1, tile_from = 0;  // the highest level built; levels [tile_from, ..) lack a pyramid kernel's copy
+  if (n_given == 1 && n_levels > 1 && f0.w[0] % 16 == 0) {
+    pyramid_l0_l1_stream_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(pool->slab[0], pool->stride[0], pool->slab[1],
+                                                                            pool->stride[1], pool->tslab[0], pool->tstride[0],
+                                                                            first, count, f0.w[0], f0.h[0], pyr_avg(ctx, f0.w[0]));
     ctx->launches++;
+    top = tile_from = 1;
+  }
+  if (int rc = tile_levels(ctx, pool, first, count, tile_from, top + 1 < n_levels ? top : n_levels)) return rc;
+  for (; top + 1 < n_levels; top += 4) {  // the fused kernel's level 0 = our level `top`
+    PyrGeom g;
+    memset(&g, 0, sizeof(g));
+    g.n_levels = n_levels - top < 5 ? n_levels - top : 5;
+    for (int l = 0; l < g.n_levels; ++l) {
+      g.w[l] = f0.w[top + l]; g.h[l] = f0.h[top + l]; g.slab[l] = pool->slab[top + l]; g.stride[l] = pool->stride[top + l];
+      g.tslab[l] = pool->tslab[top + l]; g.tstride[l] = pool->tstride[top + l];
+      if (l && pyr_avg(ctx, g.w[l - 1])) g.avg_mask |= 1u << l;
+    }
+    g.tiles_x = (g.w[0] + 127) / 128;
+    const int tiles_y = (g.h[0] + 15) / 16;
+    for (int done = 0; done < count; done += 32768) {  // gridDim.y limit 65535
+      const int n = count - done < 32768 ? count - done : 32768;
+      pyramid_fused_kernel<<<dim3(g.tiles_x * tiles_y, n), 128, 0, ctx->stream>>>(first + done, g);
+      ctx->launches++;
+    }
   }
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  if (int rc = tile_levels(ctx, fr->lv, nullptr, fr->tv, nullptr, fr->w, fr->h, tile_from, fr->n_levels, 1)) return rc;
-  if (timed) kt_end(ctx);
+  kt_end(ctx);
+  return 0;
+}
+
+// A zeroed pool of `count` frames of one geometry (arguments checked by the caller); `who` prefixes the error messages.
+static int pool_create(svo_b200_ctx* ctx, const char* who, int width, int height, int n_levels, int count,
+                       svo_b200_frame_pool** pool_out) {
+  cudaSetDevice(ctx->device);
+  svo_b200_frame proto;
+  proto.width = width; proto.height = height; proto.n_levels = n_levels;
+  svo_b200_frame_pool* pool = new svo_b200_frame_pool();
+  pool->count = count;
+  pool->n_levels = n_levels;
+  size_t total = 0, slab_off[SVO_B200_MAX_LEVELS];
+  for (int l = 0; l < n_levels; ++l) {
+    proto.w[l] = l ? proto.w[l - 1] / 2 : width;
+    proto.h[l] = l ? proto.h[l - 1] / 2 : height;
+    if (proto.w[l] <= 0 || proto.h[l] <= 0) {
+      delete pool;
+      return set_err(ctx, SVO_B200_EINVAL, "%s: level %d is empty", who, l);
+    }
+    pool->stride[l] = ((size_t)proto.w[l] * proto.h[l] + 255) / 256 * 256;
+    slab_off[l] = total;
+    total += pool->stride[l] * (size_t)count + 256;  // slack: kernels fetch aligned words around footprints
+  }
+  size_t tslab_off[SVO_B200_MAX_LEVELS];
+  for (int l = 0; l < n_levels; ++l) {
+    pool->tstride[l] = (tiled_bytes(proto.w[l], proto.h[l]) + 255) / 256 * 256;
+    tslab_off[l] = total;
+    total += pool->tstride[l] * (size_t)count;
+  }
+  cudaError_t e = cudaMalloc((void**)&pool->mem, total);
+  if (e != cudaSuccess) {
+    delete pool;
+    return set_err(ctx, SVO_B200_ENOMEM, "%s: cudaMalloc(%zu): %s", who, total, cudaGetErrorString(e));
+  }
+  cudaMemsetAsync(pool->mem, 0, total, ctx->stream);
+  for (int l = 0; l < n_levels; ++l) {
+    pool->slab[l] = pool->mem + slab_off[l];
+    pool->tslab[l] = pool->mem + tslab_off[l];
+  }
+  proto.pool = pool;
+  pool->frames.assign(count, proto);
+  for (int i = 0; i < count; ++i) {
+    pool->frames[i].index = i;
+    for (int l = 0; l < n_levels; ++l) {
+      pool->frames[i].lv[l] = pool->slab[l] + (size_t)i * pool->stride[l];
+      pool->frames[i].tv[l] = pool->tslab[l] + (size_t)i * pool->tstride[l];
+    }
+  }
+  *pool_out = pool;
   return 0;
 }
 
@@ -438,34 +484,10 @@ int svo_b200_frame_create(svo_b200_ctx* ctx, int width, int height, int n_levels
                           svo_b200_frame** frame_out) {
   if (!ctx || !frame_out || width <= 0 || height <= 0 || n_levels < 1 || n_levels > SVO_B200_MAX_LEVELS)
     return set_err(ctx, SVO_B200_EINVAL, "frame_create: bad size %dx%d levels %d", width, height, n_levels);
-  cudaSetDevice(ctx->device);
-  svo_b200_frame* fr = new svo_b200_frame();
-  fr->width = width;
-  fr->height = height;
-  fr->n_levels = n_levels;
-  size_t off = 0;
-  for (int l = 0; l < n_levels; ++l) {
-    fr->w[l] = l ? fr->w[l - 1] / 2 : width;
-    fr->h[l] = l ? fr->h[l - 1] / 2 : height;
-    if (fr->w[l] <= 0 || fr->h[l] <= 0) {
-      delete fr;
-      return set_err(ctx, SVO_B200_EINVAL, "frame_create: level %d is empty", l);
-    }
-    fr->off[l] = off;
-    off += row_major_bytes(fr->w[l], fr->h[l]) + (tiled_bytes(fr->w[l], fr->h[l]) + 255) / 256 * 256;
-  }
-  fr->bytes = off;
-  cudaError_t e = cudaMalloc((void**)&fr->base, fr->bytes);
-  if (e != cudaSuccess) {
-    delete fr;
-    return set_err(ctx, SVO_B200_ENOMEM, "frame_create: cudaMalloc(%zu): %s", off, cudaGetErrorString(e));
-  }
-  for (int l = 0; l < n_levels; ++l) {
-    fr->lv[l] = fr->base + fr->off[l];
-    fr->tv[l] = fr->lv[l] + row_major_bytes(fr->w[l], fr->h[l]);
-  }
-  cudaMemsetAsync(fr->base, 0, fr->bytes, ctx->stream);
-  *frame_out = fr;
+  svo_b200_frame_pool* pool = nullptr;
+  if (int rc = pool_create(ctx, "frame_create", width, height, n_levels, 1, &pool)) return rc;
+  pool->frames[0].owns_pool = true;
+  *frame_out = &pool->frames[0];
   return 0;
 }
 
@@ -478,7 +500,7 @@ int svo_b200_frame_upload(svo_b200_ctx* ctx, svo_b200_frame* fr, const uint8_t* 
     SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(fr->lvl(l), levels[l], (size_t)fr->w[l] * fr->h[l],
                                         cudaMemcpyHostToDevice, ctx->stream));
   }
-  return build_levels(ctx, fr, n_given, 0);
+  return build_pyramid(ctx, fr->pool, fr->index, 1, n_given);
 }
 
 int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* fr, const void* level0_dev) {
@@ -486,7 +508,7 @@ int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* fr, const vo
   cudaSetDevice(ctx->device);
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(fr->lvl(0), level0_dev, (size_t)fr->w[0] * fr->h[0],
                                       cudaMemcpyDeviceToDevice, ctx->stream));
-  return build_levels(ctx, fr, 1, 0);
+  return build_pyramid(ctx, fr->pool, fr->index, 1, 1);
 }
 
 int svo_b200_frame_download_level_tiled(svo_b200_ctx* ctx, const svo_b200_frame* fr, int level, uint8_t* out) {
@@ -510,14 +532,7 @@ int svo_b200_frame_download_level(svo_b200_ctx* ctx, const svo_b200_frame* fr, i
 }
 
 void svo_b200_frame_destroy(svo_b200_ctx* ctx, svo_b200_frame* fr) {
-  if (!fr) return;
-  if (ctx) {
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-  }
-  if (fr->pooled) return;  // borrowed handle of a pool
-  if (fr->base) cudaFree(fr->base);
-  delete fr;
+  if (fr && fr->owns_pool) svo_b200_frame_pool_destroy(ctx, fr->pool);  // else a borrowed handle of a pool
 }
 
 
@@ -525,48 +540,7 @@ int svo_b200_frame_pool_create(svo_b200_ctx* ctx, int width, int height, int n_l
                                svo_b200_frame_pool** pool_out) {
   if (!ctx || !pool_out || width <= 0 || height <= 0 || n_levels < 1 || n_levels > SVO_B200_MAX_LEVELS || count <= 0)
     return set_err(ctx, SVO_B200_EINVAL, "frame_pool_create: bad arguments");
-  cudaSetDevice(ctx->device);
-  svo_b200_frame proto;
-  proto.width = width; proto.height = height; proto.n_levels = n_levels; proto.pooled = true;
-  svo_b200_frame_pool* pool = new svo_b200_frame_pool();
-  pool->count = count;
-  pool->n_levels = n_levels;
-  size_t total = 0, slab_off[SVO_B200_MAX_LEVELS];
-  for (int l = 0; l < n_levels; ++l) {
-    proto.w[l] = l ? proto.w[l - 1] / 2 : width;
-    proto.h[l] = l ? proto.h[l - 1] / 2 : height;
-    if (proto.w[l] <= 0 || proto.h[l] <= 0) {
-      delete pool;
-      return set_err(ctx, SVO_B200_EINVAL, "frame_pool_create: level %d is empty", l);
-    }
-    pool->stride[l] = ((size_t)proto.w[l] * proto.h[l] + 255) / 256 * 256;
-    slab_off[l] = total;
-    total += pool->stride[l] * (size_t)count + 256;  // slack: kernels fetch aligned words around footprints
-  }
-  size_t tslab_off[SVO_B200_MAX_LEVELS];
-  for (int l = 0; l < n_levels; ++l) {
-    pool->tstride[l] = (tiled_bytes(proto.w[l], proto.h[l]) + 255) / 256 * 256;
-    tslab_off[l] = total;
-    total += pool->tstride[l] * (size_t)count;
-  }
-  cudaError_t e = cudaMalloc((void**)&pool->mem, total);
-  if (e != cudaSuccess) {
-    delete pool;
-    return set_err(ctx, SVO_B200_ENOMEM, "frame_pool_create: cudaMalloc(%zu): %s", total, cudaGetErrorString(e));
-  }
-  cudaMemsetAsync(pool->mem, 0, total, ctx->stream);
-  for (int l = 0; l < n_levels; ++l) {
-    pool->slab[l] = pool->mem + slab_off[l];
-    pool->tslab[l] = pool->mem + tslab_off[l];
-  }
-  pool->frames.assign(count, proto);
-  for (int i = 0; i < count; ++i)
-    for (int l = 0; l < n_levels; ++l) {
-      pool->frames[i].lv[l] = pool->slab[l] + (size_t)i * pool->stride[l];
-      pool->frames[i].tv[l] = pool->tslab[l] + (size_t)i * pool->tstride[l];
-    }
-  *pool_out = pool;
-  return 0;
+  return pool_create(ctx, "frame_pool_create", width, height, n_levels, count, pool_out);
 }
 
 svo_b200_frame* svo_b200_frame_pool_get(svo_b200_frame_pool* pool, int index) {
@@ -589,57 +563,7 @@ int svo_b200_frame_pool_upload(svo_b200_ctx* ctx, svo_b200_frame_pool* pool, int
     SVO_CUDA_CHECK(ctx, cudaMemcpy2DAsync(dst, pool->stride[0], level0_host, host_stride_bytes, img, (size_t)count,
                                           cudaMemcpyHostToDevice, ctx->stream));
   }
-  kt_begin(ctx);
-  int tiled = 0;  // levels [0, tiled) get their tiled copies from the pyramid kernels
-  if (f0.n_levels > 1) {
-    // level 0 -> 1 with the streaming kernel when the width allows 128-bit rows, then levels 2.. from
-    // level 1 with the fused tile kernel (base level shifted by one); otherwise everything from level 0.
-    const bool stream01 = (f0.w[0] % 16) == 0;
-    const int base = stream01 ? 1 : 0;
-    if (stream01) {
-      const int blocks = ctx->sm_count * 8;
-      pyramid_l0_l1_stream_kernel<<<blocks, 256, 0, ctx->stream>>>(pool->slab[0], pool->stride[0], pool->slab[1],
-                                                                   pool->stride[1], pool->tslab[0], pool->tstride[0], first,
-                                                                   count, f0.w[0], f0.h[0],
-                                                                   pyr_avg(ctx, f0.w[0]));
-      ctx->launches++;
-      tiled = 1;
-    }
-    const int n_sub = f0.n_levels - base;  // levels seen by the fused kernel, its level 0 = our level `base`
-    if (n_sub > 1) {
-      PyrGeom g;
-      memset(&g, 0, sizeof(g));
-      g.n_levels = n_sub < 5 ? n_sub : 5;
-      for (int l = 0; l < n_sub; ++l) {
-        g.w[l] = f0.w[base + l]; g.h[l] = f0.h[base + l]; g.slab[l] = pool->slab[base + l]; g.stride[l] = pool->stride[base + l];
-        g.tslab[l] = pool->tslab[base + l]; g.tstride[l] = pool->tstride[base + l];
-      }
-      for (int l = 1; l < g.n_levels; ++l)
-        if (pyr_avg(ctx, g.w[l - 1])) g.avg_mask |= 1u << l;
-      g.tiles_x = (g.w[0] + 127) / 128;
-      const int tiles_y = (g.h[0] + 15) / 16;
-      for (int done = 0; done < count; done += 32768) {  // gridDim.y limit 65535
-        const int n = count - done < 32768 ? count - done : 32768;
-        dim3 grid(g.tiles_x * tiles_y, n);
-        pyramid_fused_kernel<<<grid, 128, 0, ctx->stream>>>(first + done, g);
-        ctx->launches++;
-      }
-      tiled = base + g.n_levels;
-    }
-    SVO_CUDA_CHECK(ctx, cudaGetLastError());
-    for (int i = 0; i < count && f0.n_levels > base + 5; ++i) {  // deeper levels: plain per-level kernel
-      int rc = build_levels(ctx, &pool->frames[first + i], base + 5, f0.n_levels, false);
-      if (rc) return rc;
-    }
-  }
-  uint8_t *lv[SVO_B200_MAX_LEVELS], *tv[SVO_B200_MAX_LEVELS];
-  for (int l = 0; l < f0.n_levels; ++l) {
-    lv[l] = pool->slab[l] + (size_t)first * pool->stride[l];
-    tv[l] = pool->tslab[l] + (size_t)first * pool->tstride[l];
-  }
-  if (int rc = tile_levels(ctx, lv, pool->stride, tv, pool->tstride, f0.w, f0.h, tiled, f0.n_levels, count)) return rc;
-  kt_end(ctx);
-  return 0;
+  return build_pyramid(ctx, pool, first, count, 1);
 }
 
 void svo_b200_frame_pool_destroy(svo_b200_ctx* ctx, svo_b200_frame_pool* pool) {

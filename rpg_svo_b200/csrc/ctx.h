@@ -9,26 +9,25 @@
 #include "../../include/svo_b200.h"
 
 namespace svo {
-// Every pyramid level is stored twice: row-major (pitch == width, what the reference indexes) with 16 B of read slack
-// (kernels fetch aligned words around unaligned footprints), and as a block-tiled copy.  Block (bx, by) of the copy is 16 B:
-// rows 4by..4by+3 of columns 4bx..4bx+3, one 32-bit word per row; block-rows are ceil(W/4) blocks long and pixels outside the
-// level are zero.  Any 5x5 footprint then lies in 2x2 blocks and any 7x7 footprint in at most 3x3: the alignment kernel
-// gathers them with a few 16-byte loads instead of one or two loads per row (its gathers are priced by the number of L1
-// requests, not by bytes).  A frame keeps a pointer to each level's copy: a single frame stores it right behind the
-// row-major level, a frame pool in slabs of its own, so that the pool's row-major level-0 images stay contiguous and a
-// window of them uploads as one flat copy.
-inline size_t row_major_bytes(int W, int H) { return ((size_t)W * H + 16 + 255) / 256 * 256; }
+// Every pyramid level is stored twice: row-major (pitch == width, what the reference indexes), and as a block-tiled copy.
+// Block (bx, by) of the copy is 16 B: rows 4by..4by+3 of columns 4bx..4bx+3, one 32-bit word per row; block-rows are
+// ceil(W/4) blocks long and pixels outside the level are zero.  Any 5x5 footprint then lies in 2x2 blocks and any 7x7
+// footprint in at most 3x3: the alignment kernel gathers them with a few 16-byte loads instead of one or two loads per row
+// (its gathers are priced by the number of L1 requests, not by bytes).  Every frame lives in a frame pool (a single frame is
+// a pool of one), which keeps the tiled copies in slabs of their own, so that the pool's row-major level-0 images stay
+// contiguous and a window of them uploads as one flat copy.
 inline size_t tiled_bytes(int W, int H) { return (size_t)((W + 3) / 4) * ((H + 3) / 4) * 16; }
 }  // namespace svo
+
+struct svo_b200_frame_pool;
 
 struct svo_b200_frame {
   int width = 0, height = 0, n_levels = 0;
   int w[SVO_B200_MAX_LEVELS] = {0}, h[SVO_B200_MAX_LEVELS] = {0};
-  uint8_t* base = nullptr;  // one allocation, levels (row-major, then tiled copy) at 256-byte aligned offsets
-  size_t off[SVO_B200_MAX_LEVELS] = {0};
-  size_t bytes = 0;
-  bool pooled = false;  // memory belongs to a svo_b200_frame_pool
-  uint8_t* lv[SVO_B200_MAX_LEVELS] = {nullptr};  // level pointers (base + off[l], or into a pool's per-level slabs)
+  svo_b200_frame_pool* pool = nullptr;  // the pool holding the frame's memory, frame `index` of it
+  int index = 0;
+  bool owns_pool = false;  // made by svo_b200_frame_create: destroying the frame destroys its pool of one
+  uint8_t* lv[SVO_B200_MAX_LEVELS] = {nullptr};  // level pointers, into the pool's per-level slabs
   uint8_t* tv[SVO_B200_MAX_LEVELS] = {nullptr};  // block-tiled copies of the levels
   uint8_t* lvl(int l) const { return lv[l]; }
 };
@@ -36,10 +35,10 @@ struct svo_b200_frame {
 struct svo_b200_frame_pool {
   int count = 0;
   int n_levels = 0;
-  // one slab per pyramid level: level l of frame i at slab[l] + i*stride[l].  Level 0 of consecutive
-  // frames is contiguous up to the 256-byte rounding, so a window uploads as ONE copy (flat when the
-  // rounding adds nothing) whose rows are whole images.  The tiled copies live in slabs of their own:
-  // level l of frame i at tslab[l] + i*tstride[l].
+  // one slab per pyramid level: level l of frame i at slab[l] + i*stride[l], each slab followed by 256 B of read slack
+  // (kernels fetch aligned words around unaligned footprints).  Level 0 of consecutive frames is contiguous up to the
+  // 256-byte rounding, so a window uploads as ONE copy (flat when the rounding adds nothing) whose rows are whole images.
+  // The tiled copies live in slabs of their own: level l of frame i at tslab[l] + i*tstride[l].
   uint8_t* slab[SVO_B200_MAX_LEVELS] = {nullptr};
   size_t stride[SVO_B200_MAX_LEVELS] = {0};
   uint8_t* tslab[SVO_B200_MAX_LEVELS] = {nullptr};
