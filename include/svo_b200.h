@@ -75,7 +75,8 @@ const char* svo_b200_last_error(const svo_b200_ctx* ctx);
 void* svo_b200_stream(svo_b200_ctx* ctx);
 int svo_b200_synchronize(svo_b200_ctx* ctx);
 /* device time (CUDA events on the context's stream) of the kernel launch(es) of the most recent entry point that
- * launched any, excluding its host<->device copies; synchronises on that launch */
+ * launched any, excluding its host<->device copies; synchronises on that launch.  Runs of a staged batch that overlap the
+ * run before them (svo_b200_sia_batch_run) record no events: after back-to-back runs this is the time of the first one. */
 int svo_b200_last_kernel_ms(svo_b200_ctx* ctx, float* ms_out);
 /* number of kernels this context has launched since creation */
 uint64_t svo_b200_launch_count(const svo_b200_ctx* ctx);
@@ -173,6 +174,12 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
                              const int* feat_offset, const double* px, const double* f,
                              const double* point_pos, const uint8_t* has_point,
                              const double* ref_pos /*B*3*/);
+/* Consecutive runs of one staged batch may overlap on the device: when one CTA per pair runs (the throughput geometry of
+ * full batches) and the last work the library enqueued on the context's stream is a run of the same batch, the next run's
+ * CTAs start while the previous run's last wave drains.  Each run reads only what the stage and the frame uploads wrote, and
+ * stores its outputs after the run before it has completed, so a fetch returns the outputs of the last run.  Any other call
+ * that enqueues work (stage, fetch, uploads, the other kernels) ends the overlap.  Work of the caller's own enqueued on the
+ * context's stream between two runs must not write the frames or anything else the batch reads. */
 int svo_b200_sia_batch_run(svo_b200_ctx* ctx);
 int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out /*B*12*/, uint8_t* visible_out,
                              double* H_out /*B*36 or NULL*/, svo_b200_sia_stats* stats_out /*B or NULL*/);

@@ -385,6 +385,7 @@ static int pool_create(svo_b200_ctx* ctx, const char* who, int width, int height
     delete pool;
     return set_err(ctx, SVO_B200_ENOMEM, "%s: cudaMalloc(%zu): %s", who, total, cudaGetErrorString(e));
   }
+  ctx->sia_chain = false;
   cudaMemsetAsync(pool->mem, 0, total, ctx->stream);
   for (int l = 0; l < n_levels; ++l) {
     pool->slab[l] = pool->mem + slab_off[l];
@@ -515,6 +516,7 @@ int svo_b200_frame_download_level_tiled(svo_b200_ctx* ctx, const svo_b200_frame*
   if (!ctx || !fr || !out || level < 0 || level >= fr->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "frame_download_level_tiled: bad arguments");
   cudaSetDevice(ctx->device);
+  ctx->sia_chain = false;
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(out, fr->tv[level],
                                       tiled_bytes(fr->w[level], fr->h[level]), cudaMemcpyDeviceToHost, ctx->stream));
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
@@ -525,6 +527,7 @@ int svo_b200_frame_download_level(svo_b200_ctx* ctx, const svo_b200_frame* fr, i
   if (!ctx || !fr || !out || level < 0 || level >= fr->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "frame_download_level: bad arguments");
   cudaSetDevice(ctx->device);
+  ctx->sia_chain = false;
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(out, fr->lvl(level), (size_t)fr->w[level] * fr->h[level],
                                       cudaMemcpyDeviceToHost, ctx->stream));
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));

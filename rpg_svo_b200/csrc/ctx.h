@@ -92,6 +92,9 @@ struct svo_b200_ctx {
   int sia_scale_est = SVO_B200_SCALE_UNIT, sia_weight_fn = SVO_B200_WEIGHT_UNIT;
   bool sia_last_robust = false;   // the last alignment launch ran the robust kernel
   std::vector<float> sia_scales;  // its per-pair, per-level scales (svo_b200_sia_last_scales), fetched with its outputs
+  // The last work enqueued on `stream` is a run of the staged batch (svo_b200_sia_batch_run): the next run of that batch
+  // may then overlap it on the device.  Every other enqueue clears it (kt_begin for kernels; the copy-only entry points).
+  bool sia_chain = false;
 };
 
 namespace svo {
@@ -122,8 +125,12 @@ struct Carver {
 void sia_batch_free(svo_b200_ctx* ctx);
 void sia_split_free(svo_b200_ctx* ctx);
 // CUDA events on the context's stream bracketing the kernel launch(es) of an entry point (no copies): the live
-// per-kernel device time bench.py's roofline figures divide by
-inline void kt_begin(svo_b200_ctx* ctx) { if (ctx->ev_k0) cudaEventRecord(ctx->ev_k0, ctx->stream); }
+// per-kernel device time bench.py's roofline figures divide by.  Every entry point that launches a kernel calls kt_begin,
+// which also ends a chain of batch runs (svo_b200_ctx::sia_chain).
+inline void kt_begin(svo_b200_ctx* ctx) {
+  ctx->sia_chain = false;
+  if (ctx->ev_k0) cudaEventRecord(ctx->ev_k0, ctx->stream);
+}
 inline void kt_end(svo_b200_ctx* ctx) { if (ctx->ev_k1) cudaEventRecord(ctx->ev_k1, ctx->stream); }
 
 // Device-side camera ([EXT] vk::PinholeCamera / vk::ATANCamera): the C-ABI parameters plus the derived constants

@@ -315,6 +315,7 @@ extern "C" int svo_b200_klt_pyramid_download(svo_b200_ctx* ctx, const svo_b200_k
     return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_download: bad arguments");
   cudaSetDevice(ctx->device);
   const int w = pyr->w[level], h = pyr->h[level], S = w + 2 * kB;
+  ctx->sia_chain = false;
   if (img_out)
     SVO_CUDA_CHECK(ctx, cudaMemcpy2DAsync(img_out, w, pyr->img[level] + (size_t)kB * S + kB, S, w, h, cudaMemcpyDeviceToHost, ctx->stream));
   if (deriv_out)

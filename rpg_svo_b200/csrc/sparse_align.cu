@@ -525,6 +525,12 @@ __device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 constexpr int kHsumBarrier = 1;  // the level's H partials (one CTA per pair)
 
+// Programmatic dependent launch.  launch_dependents: once every CTA of this grid has executed it, a grid launched after it
+// with cudaLaunchAttributeProgrammaticStreamSerialization may start its CTAs in the slots this grid's CTAs free.  wait: returns
+// once the grid this one depends on has completed and its memory writes are visible (at once when launched without the attribute).
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // Sum of the 21 unique H entries + one count over the per-feature moments of the whole pair, once per level
 // (and in the rare "slow path"): per-warp partials, one shared-memory hop, warp 0 adds the per-warp partials (and, in the
 // cluster variant, the per-CTA sums every CTA received through DSMEM, after a cluster barrier).  On return the totals are in
@@ -847,6 +853,10 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   // features of this CTA: [fbase, min(N, fbase + S)); their records are np_loc padded entries of the pair's blob
   const int n_loc = max(0, min(N - fbase, S));
   const int np_loc = (n_loc + 15) & ~15;
+
+  // Throughput geometry: the next run of the same staged batch (svo_b200_sia_batch_run) may start its CTAs while this
+  // launch's last wave drains; it reads nothing this launch writes, and orders its output stores after this launch (below).
+  if constexpr (SS && !EVAL) griddep_launch_dependents();
 
   if (tid == 0) {
     mbar_init(&s.mbar, 1);
@@ -1573,6 +1583,10 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   if constexpr (UP) pair_sync<CS>();  // no CTA of the cluster exits while another may still write into its shared memory
 
   // ---- outputs ---------------------------------------------------------------------------------
+  // Launched as a dependent of the previous run of its batch, this launch writes the same outputs: wait for that run to
+  // complete.  These are the first global stores of the instantiation (the iteration trace is written only by the
+  // single-pair svo_b200_sparse_img_align, whose launch is never a dependent).
+  if constexpr (SS && !EVAL) griddep_wait();
 #pragma unroll
   for (int k = 0; k < FPT; ++k) {
     const int i = tid + k * T;
@@ -2167,7 +2181,12 @@ static int pick_launch(svo_b200_ctx* ctx, int B, int max_feat, int n_lvl, const 
 // Launches geometry `geo` (from pick_launch) and records the launch for svo_b200_sia_last_launch.  The undistorted pinhole
 // runs the geometry's plain-pinhole instantiation where it has one; the residual pass (eval) runs its general-camera,
 // per-level instantiation.
-static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, const SiaEntry& geo, size_t smem, bool eval) {
+// `chain`: the last work on the stream is a run of the same staged batch.  The throughput geometry then launches as its
+// programmatic dependent -- its CTAs fill the slots the previous run's last wave frees, and wait for that run before they
+// store the outputs -- without the kernel-time events, whose records between the two kernels would serialise them again.
+// The other geometries run few CTAs per SM or small batches, where an overlap would shorten the time per launch and not a
+// pair's latency: they are never chained.
+static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, const SiaEntry& geo, size_t smem, bool eval, bool chain) {
   const bool plain = !eval && !P.cam.distorted && P.cam.model == SVO_B200_CAM_PINHOLE;
   const SiaEntry* e = sia_variant(geo, !plain, geo.upfront && !eval);
   if (!e) e = &geo;
@@ -2181,16 +2200,24 @@ static int launch_sia(svo_b200_ctx* ctx, const SiaParams& P, int B, const SiaEnt
   cfg.blockDim = dim3((unsigned)e->threads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = ctx->stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)e->cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  const bool dependent = chain && !eval && e->throughput;
+  cudaLaunchAttribute attr[2];
   cfg.attrs = attr;
-  cfg.numAttrs = e->cluster > 1 ? 1 : 0;
-  kt_begin(ctx);
+  if (e->cluster > 1) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+    attr[cfg.numAttrs].val.clusterDim.x = (unsigned)e->cluster;
+    attr[cfg.numAttrs].val.clusterDim.y = 1;
+    attr[cfg.numAttrs].val.clusterDim.z = 1;
+    cfg.numAttrs++;
+  }
+  if (dependent) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    cfg.numAttrs++;
+  }
+  if (!dependent) kt_begin(ctx);
   SVO_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, kern, P));
-  kt_end(ctx);
+  if (!dependent) kt_end(ctx);
   ctx->launches++;
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
   svo_b200_sia_launch& L = ctx->sia_last;  // what ran, for svo_b200_sia_last_launch
@@ -2396,6 +2423,7 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
   if (!ctx->sia) ctx->sia = new SiaBatchState();
   SiaBatchState& st = *ctx->sia;
   st.staged = false;
+  ctx->sia_chain = false;
   st.B = B;
   st.total_feat = feat_offset[B] - feat_offset[0];
   st.max_feat = 0;
@@ -2500,8 +2528,9 @@ int svo_b200_sia_batch_run(svo_b200_ctx* ctx) {
   if (!ctx || !ctx->sia || !ctx->sia->staged) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_run: nothing staged");
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
-  if (st.robust_weight >= 0) return launch_sia_robust(ctx, st);
-  return launch_sia(ctx, st.P, st.B, *st.geo, st.smem, false);
+  const int rc = st.robust_weight >= 0 ? launch_sia_robust(ctx, st) : launch_sia(ctx, st.P, st.B, *st.geo, st.smem, false, ctx->sia_chain);
+  ctx->sia_chain = rc == 0;
+  return rc;
 }
 
 int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_out, double* H_out,
@@ -2509,6 +2538,7 @@ int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_
   if (!ctx || !ctx->sia || !ctx->sia->staged) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_fetch: nothing staged");
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
+  ctx->sia_chain = false;
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(st.h_out.p, st.d_out.p, st.out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
   SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
   if (ctx->xg_connected) {  // did every peer take part in every exchange?
@@ -2606,7 +2636,7 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
   st.P.Jres_out = reinterpret_cast<double*>(ds + o_j);
   st.P.chi2_out = reinterpret_cast<double*>(ds + o_c);
   st.P.n_meas_out = reinterpret_cast<long long*>(ds + o_n);
-  if ((rc = launch_sia(ctx, st.P, 1, *st.geo, st.smem, true))) return rc;
+  if ((rc = launch_sia(ctx, st.P, 1, *st.geo, st.smem, true, false))) return rc;
   double Tdummy[12];
   if ((rc = svo_b200_sia_batch_fetch(ctx, Tdummy, visible_io, H_out, nullptr))) return rc;
   if (ref_patch_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(ref_patch_out, ds + o_rp, sizeof(float) * 16 * (size_t)N, cudaMemcpyDeviceToHost));
