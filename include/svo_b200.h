@@ -131,7 +131,7 @@ void svo_b200_frame_pool_destroy(svo_b200_ctx* ctx, svo_b200_frame_pool* pool);
 /* ------------------------------------------------------------------ SparseImgAlign ------ */
 typedef struct {
   int max_level, min_level; /* coarsest / finest pyramid level (ctor args) */
-  int n_iter;               /* max GN iterations per level */
+  int n_iter;               /* max GN iterations per level (< 0: 1000, the reference's unbounded size_t) */
   double eps;               /* convergence threshold on |x|_inf; reference: 1e-6 */
 } svo_b200_sia_options;
 

@@ -115,7 +115,8 @@ def sparse_img_align(ref_pyr, cur_pyr, cam, T_init, px, f, pos, has_point, ref_p
     visible = np.zeros(max(n, 1), dtype=np.uint8)
     H = np.zeros(36)
     res = np.zeros((max(n, 1), 16), dtype=np.float32)
-    cap = (max_level - min_level + 1) * max(n_iter, 1) + 8
+    # a negative n_iter is the reference's size_t n_iter_ wrapped around: no limit (room for 100 per level)
+    cap = (max_level - min_level + 1) * (max(n_iter, 1) if n_iter >= 0 else 100) + 8
     trace = (SiaIter * cap)()
     ntr = C.c_int(0)
     cs = cam_struct(cam)

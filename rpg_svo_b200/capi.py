@@ -270,7 +270,9 @@ class Context:
         visible = np.zeros(max(n, 1), np.uint8)
         H = np.zeros(36)
         stats = SiaStats()
-        cap = ((max_level - min_level + 1) * max(n_iter, 1) + 8) if want_trace else 0
+        # a negative n_iter runs up to 1000 iterations per level (the reference's size_t n_iter_: no limit); the trace
+        # has room for 100 per level
+        cap = ((max_level - min_level + 1) * (max(n_iter, 1) if n_iter >= 0 else 100) + 8) if want_trace else 0
         trace = (SiaIter * cap)() if cap else None
         ntr = C.c_int(0)
         cs = cam_struct(cam)

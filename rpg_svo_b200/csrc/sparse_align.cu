@@ -1448,11 +1448,14 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         if constexpr (!SS) patch_moments(pat_dxy, in_mask, q_sxx, q_sxy, q_syy);
         pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
             [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
+              // a feature outside the image contributes nothing, also where its Jacobian rows are not finite (a point at
+              // zero depth, or with f_z == 0): 1/z is selected away, the rows are then finite and the moments zero
               { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); }
               if constexpr (SS) feat_moments(pat_dxy, in_mask, k, sxx, sxy, syy);
               else { sxx = sel_k(q_sxx, k); sxy = sel_k(q_sxy, k); syy = sel_k(q_syy, k); }
               cnt = 0.0;
               asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));  // see the per-level call: no hoisting into local memory
+              if (!((in_mask >> k) & 1u)) zi = 0.0;
             },
             s, nwarps, P.xg, pair);
       };
@@ -2056,6 +2059,9 @@ struct SiaBatchState {
   int robust_weight = -1;
   int robust_slots = 0;
   size_t o_scales = 0;
+  // features whose xyz_ref is not finite (sia_kernel only): staged without their point, visibility as the reference has it
+  struct Nonfinite { int feat, pair, vis_levels; };  // vis_levels: the levels the set-only mask holds it at
+  std::vector<Nonfinite> nonfinite;
 };
 
 void sia_batch_free(svo_b200_ctx* ctx) {
@@ -2265,6 +2271,38 @@ static int launch_sia_robust(svo_b200_ctx* ctx, const SiaBatchState& st) {
 
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
 
+// A point whose xyz_ref = f * |pos - ref_pos| is not finite projects to NaN at every pose: the reference keeps it visible
+// where its reference patch fits, and it never enters a residual pass.  sia_kernel, which sums every visible feature's
+// Jacobian rows times its moments (zero where the feature is not in the image), would turn 0 * NaN into a NaN normal matrix:
+// such features are staged as a slot without a point at a finite position, and their visibility is the reference's border
+// test (precomputeReferencePatches, sparse_img_align.cpp:84-99), counted in the pair's sum_visible as the kernel counts.
+static bool finite_xyz_ref(const double* f, const double* pos, const double* ref_pos) {
+  // every input finite (the common case): 0 * (a sum of them) is 0, where any is inf or NaN it is NaN
+  if (std::isfinite(0.0 * (f[0] + f[1] + f[2] + pos[0] + pos[1] + pos[2] + ref_pos[0] + ref_pos[1] + ref_pos[2]))) {
+    const double m = fmax(fmax(fabs(pos[0] - ref_pos[0]), fabs(pos[1] - ref_pos[1])), fabs(pos[2] - ref_pos[2]));
+    if (m < 1e150) return true;  // no overflow in the depth either
+  }
+  const double dx = pos[0] - ref_pos[0], dy = pos[1] - ref_pos[1], dz = pos[2] - ref_pos[2];
+  const double depth = sqrt(dx * dx + dy * dy + dz * dz);
+  return std::isfinite(f[0] * depth) && std::isfinite(f[1] * depth) && std::isfinite(f[2] * depth);
+}
+// The number of levels (max..min) at which the set-only visibility mask holds a feature: from the first level its reference
+// patch fits on.  0: never visible.
+static int ref_patch_levels(const double* px, const SiaParams& P, const svo_b200_frame* ref) {
+  int n = 0;
+  bool vis = false;
+  for (int l = P.max_level; l >= P.min_level; --l) {
+    const float scale = 1.0f / (float)(1 << l);
+    const float u = (float)(px[0] * scale), v = (float)(px[1] * scale);
+    if (u >= 0.f && v >= 0.f && u < 1e6f && v < 1e6f) {
+      const int ui = (int)floorf(u), vi = (int)floorf(v);
+      vis = vis || (ui - 3 >= 0 && vi - 3 >= 0 && ui + 3 < ref->w[l] && vi + 3 < ref->h[l]);
+    }
+    n += vis ? 1 : 0;
+  }
+  return n;
+}
+
 // Pack one pair's features into the blob layout the kernel stages with TMA.
 static void pack_blob(uint8_t* dst, int n, int np, const double* px, const double* f, const double* pos,
                       const uint8_t* hp) {
@@ -2276,6 +2314,8 @@ static void pack_blob(uint8_t* dst, int n, int np, const double* px, const doubl
   memcpy(dst + (size_t)np * 64, hp, n);
 }
 
+constexpr int kSiaUnboundedIters = 1000;  // iterations per level for a negative n_iter
+
 static int fill_common(svo_b200_ctx* ctx, SiaParams& P, const svo_b200_frame* fr, const svo_b200_camera* cam,
                        const svo_b200_sia_options* opt) {
   memset(&P, 0, sizeof(P));
@@ -2285,7 +2325,11 @@ static int fill_common(svo_b200_ctx* ctx, SiaParams& P, const svo_b200_frame* fr
   for (int l = 0; l < fr->n_levels; ++l) { P.w[l] = fr->w[l]; P.h[l] = fr->h[l]; }
   int rc = cam_to_dev(ctx, cam, P.cam);
   if (rc) return rc;
-  P.max_level = opt->max_level; P.min_level = opt->min_level; P.n_iter = opt->n_iter; P.eps = opt->eps;
+  P.max_level = opt->max_level; P.min_level = opt->min_level; P.eps = opt->eps;
+  // The reference's n_iter_ is a size_t: a negative n_iter wraps around to no limit.  Here it is kSiaUnboundedIters per level,
+  // which no converging level reaches, while a level that never stops (no measurement or a zero residual, with a NaN or
+  // negative eps) ends within milliseconds instead of running for hours.  The robust kernel takes the same bound.
+  P.n_iter = opt->n_iter < 0 ? kSiaUnboundedIters : opt->n_iter;
   P.debug = getenv("SVO_B200_SIA_DEBUG") ? 1 : 0;
   P.xg.rank = 0; P.xg.world = 1;
   if (ctx->xg_connected) {
@@ -2427,6 +2471,7 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
   st.B = B;
   st.total_feat = feat_offset[B] - feat_offset[0];
   st.max_feat = 0;
+  st.nonfinite.clear();
   for (int b = 0; b < B; ++b) {
     const int n = feat_offset[b + 1] - feat_offset[b];
     if (n < 0) return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: feat_offset not monotone");
@@ -2491,6 +2536,18 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
     memcpy(j.ref_pos, ref_pos + 3 * (size_t)b, sizeof(double) * 3);
     if (n > 0) pack_blob(hin + o_blob[b], n, j.n_pad, px + 2 * (size_t)o, f + 3 * (size_t)o,
                          point_pos + 3 * (size_t)o, has_point + o);
+    if (!weighted)
+      for (int i = 0; i < n; ++i)
+        if (has_point[o + i] && !finite_xyz_ref(f + 3 * (size_t)(o + i), point_pos + 3 * (size_t)(o + i), ref_pos + 3 * (size_t)b)) {
+          double* d = reinterpret_cast<double*>(hin + o_blob[b]);
+          const double* rp = ref_pos + 3 * (size_t)b;
+          for (int c = 0; c < 3; ++c) {  // the neutral xyz_ref (0, 0, ~1) of a slot without a feature
+            d[2 * (size_t)j.n_pad + 3 * i + c] = c == 2 ? 1.0 : 0.0;
+            d[5 * (size_t)j.n_pad + 3 * i + c] = c == 2 ? rp[c] + 1.0 : rp[c];
+          }
+          hin[o_blob[b] + (size_t)j.n_pad * 64 + i] = 0;
+          st.nonfinite.push_back({j.feat_off + i, b, ref_patch_levels(px + 2 * (size_t)(o + i), st.P, ref[b])});
+        }
   }
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(din, hin, st.in_bytes, cudaMemcpyHostToDevice, ctx->stream));
 
@@ -2553,6 +2610,18 @@ int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_
   if (H_out) memcpy(H_out, h + st.o_H, sizeof(double) * 36 * (size_t)st.B);
   if (stats_out) memcpy(stats_out, h + st.o_stats, sizeof(svo_b200_sia_stats) * (size_t)st.B);
   if (visible_out) memcpy(visible_out, h + st.o_vis, (size_t)st.total_feat);
+  if (st.P.n_iter == 0 && st.robust_weight < 0) {
+    // no iteration: SparseImgAlign computes the reference patches, and so the visibility, only inside the first residual
+    // pass (the robust cost's scale pass at the start pose computes them there): no feature is visible at any level
+    if (visible_out) memset(visible_out, 0, (size_t)st.total_feat);
+    if (stats_out)
+      for (int b = 0; b < st.B; ++b) stats_out[b].sum_visible = 0;
+  } else {
+    for (const auto& q : st.nonfinite) {  // the points staged without their position (finite_xyz_ref)
+      if (visible_out) visible_out[q.feat] = q.vis_levels > 0;
+      if (stats_out) stats_out[q.pair].sum_visible += q.vis_levels;
+    }
+  }
   if (st.robust_weight >= 0 && ctx->sia_last_robust && ctx->sia_scales.size() == (size_t)st.B * SVO_B200_MAX_LEVELS)
     memcpy(ctx->sia_scales.data(), h + st.o_scales, sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)st.B);
   return 0;
