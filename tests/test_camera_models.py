@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from rpg_svo_b200 import synth
+from tests import depth_update_hp as dhp
 from tests.ref_golden import ref, with_patch_digest  # noqa: F401 (ref: fixture)
 
 CAMERAS = ["atan", "pinhole_radtan"]
@@ -128,8 +129,7 @@ def test_gpu_depth_filter_distorted(ctx, oracle, kind):
     assert upd.sum() > 0.25 * len(upd)
     assert np.max(np.abs(g["px_cur"][upd] - o["px_cur"][upd])) <= 1e-4
     assert np.allclose(g["z"][upd], o["z"][upd], rtol=1e-6)
-    for k in ("a", "b", "mu", "sigma2"):
-        assert np.allclose(g[k], o[k], rtol=2e-5, atol=1e-7), k
+    dhp.assert_seed_updates(g, o, c["seeds"], [c["T_ref_w"]], c["ref_index"], c["T_cur_w"], c["ftr_f"], cam.fx, oracle)
     ref.destroy(); cur.destroy()
 
 

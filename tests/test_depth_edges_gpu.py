@@ -5,7 +5,9 @@ compiled reference's recorded outputs."""
 import numpy as np
 import pytest
 
+from oracle import binding
 from rpg_svo_b200 import synth
+from tests import depth_update_hp as hp
 from tests.ref_golden import RefCalls
 
 pytestmark = pytest.mark.gpu
@@ -18,15 +20,16 @@ def _bits(x):
     return np.ascontiguousarray(x, np.float32).view(np.uint32)
 
 
-def _check_update(g, o, min_updated=0):
-    """status and n_zmssd bit-exact; seeds that never reach updateSeed bit-identical; updated seeds to expf's rounding."""
+def _check_update(g, o, c, kf_T, min_updated=0, oracle_statement=True):
+    """status and n_zmssd bit-exact; seeds that never reach updateSeed bit-identical; every updated seed of the kernel
+    bit for bit one of the exactly rounded statement's candidates from its own depth (tests/depth_update_hp.py: only
+    expf, computeTau's acos / sin / atan and the pose product are left open), and the oracle's bit for bit its own."""
     assert np.array_equal(g["status"], o["status"])
     assert np.array_equal(g["n_zmssd"], o["n_zmssd"])
     upd = o["status"] >= UPDATED
     assert upd.sum() >= min_updated
-    for k in SEED_KEYS:
-        assert np.array_equal(_bits(g[k][~upd]), _bits(o[k][~upd])), k
-        assert np.allclose(g[k][upd], o[k][upd], rtol=2e-5, atol=1e-7), k
+    hp.assert_seed_updates(g, o, c["seeds"], kf_T, c["ref_index"], c["T_cur_w"], c["ftr_f"], c["cam"].fx, binding,
+                           oracle_statement=oracle_statement)
     assert np.max(np.abs(g["px_cur"][upd] - o["px_cur"][upd]), initial=0.0) <= 1e-4
     assert np.allclose(g["z"][upd], o["z"][upd], rtol=1e-6)
 
@@ -55,7 +58,7 @@ def test_depth_filter_two_keyframes_vs_oracle_and_reference(ctx, oracle):
     kf_pyr, kf_T = [a["ref_pyr"], b["ref_pyr"]], [a["T_ref_w"], b["T_ref_w"]]
     c = dict(a, ref_index=ref_index, ftr_type=ftr_type)
     g, o = _run_both(ctx, oracle, kf_pyr, kf_T, c)
-    _check_update(g, o, min_updated=50)
+    _check_update(g, o, c, kf_T, min_updated=50)
     r = RefCalls("test_oracle_pins", "test_oracle_depth_filter_two_keyframes_equals_reference_source_compiled_here")
     rr = r.depth_filter_update([k[0] for k in kf_pyr], kf_T, a["cur_pyr"][0], a["T_cur_w"], a["n_levels"], a["cam"],
                                ref_index, a["ftr_px"], a["ftr_f"], a["ftr_level"], ftr_type, a["ftr_grad"], a["batch_id"],
@@ -76,7 +79,7 @@ def test_depth_filter_interleaved_keyframes(ctx, oracle, n_kfs):
     another keyframe's image or pose than ref_index names would scan the wrong patch along the wrong line."""
     c = synth.make_multi_keyframe_depth_case(70 + n_kfs, n_seeds=400, n_kfs=n_kfs)
     g, o = _run_both(ctx, oracle, c["kf_pyr"], c["kf_T"], c)
-    _check_update(g, o, min_updated=100)
+    _check_update(g, o, c, c["kf_T"], min_updated=100)
     upd = o["status"] >= UPDATED
     for r in range(n_kfs):  # every keyframe's seeds are measured, near their own true depth
         m = upd & (c["ref_index"] == r)
@@ -90,7 +93,7 @@ def test_depth_filter_every_seed_status(ctx, oracle):
     NaN or infinite, against the oracle and the reference's outputs recorded by test_edge_pins.py."""
     c = synth.make_seed_status_case(91)
     g, o = _run_both(ctx, oracle, [c["ref_pyr"]], [c["T_ref_w"]], c)
-    _check_update(g, o, min_updated=50)
+    _check_update(g, o, c, [c["T_ref_w"]], min_updated=50)
     st = g["status"]
     counts = {s: int((st == s).sum()) for s in range(1, 8)}
     print("seed statuses (1 too old .. 6 converged, 7 NaN):", counts)
@@ -121,9 +124,9 @@ def test_depth_filter_search_step_limit(ctx, oracle, limit):
     default of 1000) are exactly skipped scans -- NO_MATCH with no score -- and there are some."""
     c = synth.make_depth_case(33, n_seeds=1500, baseline=0.3)
     g, o = _run_both(ctx, oracle, [c["ref_pyr"]], [c["T_ref_w"]], c, max_epi_search_steps=limit)
-    _check_update(g, o)
+    _check_update(g, o, c, [c["T_ref_w"]], oracle_statement=False)
     gd, od = _run_both(ctx, oracle, [c["ref_pyr"]], [c["T_ref_w"]], c)
-    _check_update(gd, od)
+    _check_update(gd, od, c, [c["T_ref_w"]], oracle_statement=False)
     changed = (g["status"] != gd["status"]) | (g["n_zmssd"] != gd["n_zmssd"])
     assert changed.sum() > 0
     assert np.all(g["status"][changed] == NO_MATCH) and np.all(g["n_zmssd"][changed] == 0)

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 
 from rpg_svo_b200 import synth
+from tests import depth_update_hp as dhp
 from tests import point_hp
 
 pytestmark = pytest.mark.gpu
@@ -90,8 +91,7 @@ def test_depth_filter_update_matches_oracle(ctx, oracle, n_seeds, baseline):
     assert upd.sum() > 0.3 * n_seeds
     assert np.max(np.abs(g["px_cur"][upd] - o["px_cur"][upd])) <= 1e-4
     assert np.allclose(g["z"][upd], o["z"][upd], rtol=1e-6)
-    for k in ("a", "b", "mu", "sigma2"):
-        assert np.allclose(g[k], o[k], rtol=2e-5, atol=1e-7), k
+    dhp.assert_seed_updates(g, o, c["seeds"], [c["T_ref_w"]], c["ref_index"], c["T_cur_w"], c["ftr_f"], c["cam"].fx, oracle)
     # the measurements are real: triangulated depth close to the plane depth
     assert np.median(np.abs(g["z"][upd] - c["depth_gt"][upd])) < 0.05
     ref.destroy(); cur.destroy()

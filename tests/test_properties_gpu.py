@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from rpg_svo_b200 import capi, synth
+from tests import depth_update_hp as hp
 
 pytestmark = pytest.mark.gpu
 B, W, H, NFEAT, NLEV = 592, 640, 480, 300, 5
@@ -91,23 +92,45 @@ def test_window_invariant_to_the_world_frame(ctx, window):
     assert np.array_equal(a["visible"], b["visible"])
 
 
-def test_depth_filter_contracts_over_a_sequence(ctx):
+def test_depth_filter_contracts_over_a_sequence(ctx, oracle):
     """Seeds initialised as in DepthFilter::initializeSeeds (mu = 1/2 m, sigma = range/6) and updated with ten frames
-    on a widening baseline: the variance never grows, converged seeds sit at the true depth."""
+    on a widening baseline: the variance never grows, converged seeds sit at the true depth.  At every step, and on a
+    frame at sub-pixel parallax (4 mm from the keyframe) applied to the initial seeds, every fifth updated seed is one of
+    the exactly rounded statement's candidates for the kernel's own inputs (tests/depth_update_hp.py).  The oracle runs
+    the same sequence on its own seeds; how far the two drift apart is printed, not asserted (expf and computeTau's
+    transcendentals differ)."""
     c = synth.make_depth_case(77, n_seeds=1500, baseline=0.05)
     ref = ctx.frame(c["ref_pyr"])
     seeds = {k: v.copy() for k, v in c["seeds"].items()}
+    o_seeds = {k: v.copy() for k, v in c["seeds"].items()}
     alive = np.ones(c["M"], bool)
     conv_err = []
     plane, tex = synth.Plane.tilted(), synth.make_texture(7)
     rng = np.random.default_rng(5)
+    every5 = np.arange(c["M"]) % 5 == 0
+    a = (c["ref_index"], c["ftr_px"], c["ftr_f"], c["ftr_level"], c["ftr_type"], c["ftr_grad"], np.full(c["M"], 5, np.int32), 6)
+    checked = ill = 0
+
+    def frame(xi):
+        T_cur = synth.se3_mul(synth.se3_exp(xi), c["T_ref_w"])
+        return T_cur, synth.build_pyramid(synth.render(c["cam"], T_cur, plane, tex), c["n_levels"])
+
+    def kernel(T_cur, cur_pyr, seeds_in):
+        nonlocal checked, ill
+        cur = ctx.frame(cur_pyr)
+        g = ctx.depth_filter_update([ref], [c["T_ref_w"]], cur, T_cur, c["cam"], *a, seeds_in)
+        cur.destroy()
+        rep = hp.check_launch(g, seeds_in, [c["T_ref_w"]], c["ref_index"], T_cur, c["ftr_f"], c["cam"].fx, only=every5)
+        assert not rep["bad"], rep["bad"][:3]
+        checked, ill = checked + rep["n"], ill + rep["ill"]
+        return g
+
+    kernel(*frame(np.concatenate([[0.004, 0.001, 0.0], np.deg2rad([0.2, -0.1, 0.1])])), seeds)  # sub-pixel parallax
     for step in range(10):
         xi = np.concatenate([rng.normal(size=3) * [1, 1, 0.2] * (0.04 + 0.03 * step), np.deg2rad(rng.uniform(-1, 1, 3))])
-        T_cur = synth.se3_mul(synth.se3_exp(xi), c["T_ref_w"])
-        cur = ctx.frame(synth.build_pyramid(synth.render(c["cam"], T_cur, plane, tex), c["n_levels"]))
-        g = ctx.depth_filter_update([ref], [c["T_ref_w"]], cur, T_cur, c["cam"], c["ref_index"], c["ftr_px"], c["ftr_f"],
-                                    c["ftr_level"], c["ftr_type"], c["ftr_grad"], np.full(c["M"], 5, np.int32), 6, seeds)
-        cur.destroy()
+        T_cur, cur_pyr = frame(xi)
+        g = kernel(T_cur, cur_pyr, seeds)
+        o = oracle.depth_filter_update([c["ref_pyr"]], [c["T_ref_w"]], cur_pyr, T_cur, c["cam"], *a, o_seeds)
         upd = alive & (g["status"] >= 5)
         assert np.all(g["sigma2"][upd] <= seeds["sigma2"][upd] * (1 + 1e-6))                   # information only accumulates
         conv = alive & (g["status"] == 6)
@@ -115,5 +138,13 @@ def test_depth_filter_contracts_over_a_sequence(ctx):
         alive &= ~np.isin(g["status"], (6, 7))
         for k in ("a", "b", "mu", "sigma2"):
             seeds[k] = np.where(alive, g[k], seeds[k]).astype(np.float32)
+            o_seeds[k] = np.where(alive, o[k], o_seeds[k]).astype(np.float32)
+        both = alive & np.isfinite(seeds["mu"]) & np.isfinite(o_seeds["mu"])
+        rel = np.abs(seeds["mu"][both] - o_seeds["mu"][both]) / np.abs(o_seeds["mu"][both])
+        print(f"step {step}: kernel/oracle free-running divergence of mu: max {rel.max(initial=0):.3g} relative, "
+              f"{int(np.sum(seeds['mu'][both] != o_seeds['mu'][both]))} of {int(both.sum())} seeds differ; "
+              f"status differs on {int(np.sum(g['status'] != o['status']))}")
     ref.destroy()
+    print(f"candidate check: {checked} updated seeds, {ill} ill-conditioned")
+    assert checked > 500
     assert len(conv_err) > 300 and np.median(conv_err) < 0.02                                  # metres at ~2 m depth

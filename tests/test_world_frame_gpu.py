@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from rpg_svo_b200 import synth
+from tests import depth_update_hp as dhp
 from tests import world_frame_cases as wf
 
 pytestmark = pytest.mark.gpu
@@ -289,14 +290,15 @@ def test_find_match_direct_in_every_frame(ctx, oracle, scenes):
 
 
 def test_depth_filter_in_every_frame(ctx, oracle, scenes):
-    """(b) status and ZMSSD counts exact, seeds within 2e-5 relative of the oracle; (c) against the canonical run."""
-    runs = [(fid, *_depth_runs(ctx, oracle, c, scenes["depth_frames"])) for fid, _, c in _frames_for("depth", scenes)]
-    _, g0, o0 = runs[0]
+    """(b) status and ZMSSD counts exact, every updated seed bit for bit one of the exactly rounded statement's candidates
+    (tests/depth_update_hp.py); (c) against the canonical run."""
+    runs = [(fid, c, *_depth_runs(ctx, oracle, c, scenes["depth_frames"])) for fid, _, c in _frames_for("depth", scenes)]
+    _, _, g0, o0 = runs[0]
     worst, edges = 0.0, 0
-    for fid, g, o in runs:
+    for fid, c, g, o in runs:
         assert np.array_equal(g["status"], o["status"]) and np.array_equal(g["n_zmssd"], o["n_zmssd"]), fid
-        for k in ("a", "b", "mu", "sigma2"):
-            assert np.allclose(g[k], o[k], rtol=2e-5, atol=1e-7), (fid, k)
+        dhp.assert_seed_updates(g, o, c["seeds"], [c["T_ref_w"]], c["ref_index"], c["T_cur_w"], c["ftr_f"], c["cam"].fx,
+                                oracle, oracle_statement=False)
         if not _exact(fid):
             continue
         flips = _flips(g["status"], g0["status"])
