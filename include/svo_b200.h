@@ -56,7 +56,10 @@ typedef struct svo_b200_frame svo_b200_frame;
  *   SVO_B200_CAM_ATAN     vk::ATANCamera(width, height, fx, fy, cx, cy, s) (PTAM's FOV model): fx, fy, cx, cy are the
  *                         PIXEL values the vikit constructor derives (fx_ = width*fx, cx_ = width*cx - 0.5, ...),
  *                         d[0] = s (0 = no distortion).
- * Zero-initialising model and d gives the undistorted pinhole camera. */
+ * Zero-initialising model and d gives the undistorted pinhole camera.
+ * width x height must be the level-0 size of every frame a call hands with the camera (the current frame, the keyframes;
+ * for the streams calls, each stream's current frame and the keyframes its seeds refer to), as svo::Frame requires
+ * (svo/src/frame.cpp:51): every entry point that takes a camera returns SVO_B200_EINVAL otherwise, before any work. */
 #define SVO_B200_CAM_PINHOLE 0
 #define SVO_B200_CAM_ATAN 1
 typedef struct {

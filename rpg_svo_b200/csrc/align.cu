@@ -181,6 +181,8 @@ int svo_b200_find_match_direct(svo_b200_ctx* ctx, const svo_b200_frame* const* r
   if (opt->max_search_level >= cur->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: max_search_level %d >= %d pyramid levels",
                    opt->max_search_level, cur->n_levels);
+  if (const int rc_sz = cam_check_frames(ctx, "find_match_direct", cam, &cur, 1)) return rc_sz;
+  if (const int rc_sz = cam_check_frames(ctx, "find_match_direct", cam, ref_frames, n_ref)) return rc_sz;
   cudaSetDevice(ctx->device);
   Carver c;
   const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),

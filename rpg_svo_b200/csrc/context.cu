@@ -59,6 +59,17 @@ int cam_to_dev(svo_b200_ctx* ctx, const svo_b200_camera* cam, CamDev& o) {
   return 0;
 }
 
+// svo::Frame refuses an image whose size is not its camera's (svo/src/frame.cpp:51), and the kernels bound their image reads
+// by the camera's size: a camera whose size is not the level-0 size of each of the n frames is refused (NULL entries are the
+// caller's to check).
+int cam_check_frames(svo_b200_ctx* ctx, const char* who, const svo_b200_camera* cam, const svo_b200_frame* const* frames, int n) {
+  for (int i = 0; i < n; ++i)
+    if (frames[i] && (frames[i]->width != cam->width || frames[i]->height != cam->height))
+      return set_err(ctx, SVO_B200_EINVAL, "%s: camera %dx%d, frame %dx%d", who, cam->width, cam->height, frames[i]->width,
+                     frames[i]->height);
+  return 0;
+}
+
 int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes) {
   if (bytes <= b.cap) return 0;
   if (b.p) {

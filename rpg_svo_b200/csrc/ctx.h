@@ -144,5 +144,6 @@ struct CamDev {
   int width, height;
 };
 int cam_to_dev(svo_b200_ctx* ctx, const svo_b200_camera* cam, CamDev& out);
+int cam_check_frames(svo_b200_ctx* ctx, const char* who, const svo_b200_camera* cam, const svo_b200_frame* const* frames, int n);
 
 }  // namespace svo

@@ -499,6 +499,8 @@ extern "C" int svo_b200_depth_filter_update(svo_b200_ctx* ctx, const svo_b200_fr
   if (opt->max_search_level >= cur->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: max_search_level %d >= %d pyramid levels",
                    opt->max_search_level, cur->n_levels);
+  if (const int rc = cam_check_frames(ctx, "depth_filter_update", cam, &cur, 1)) return rc;
+  if (const int rc = cam_check_frames(ctx, "depth_filter_update", cam, ref_frames, n_ref)) return rc;
   DepthStream st;
   if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, batch_counter, st)) return rc;
   const int seed_offset[2] = {0, M};
@@ -546,6 +548,13 @@ extern "C" int svo_b200_depth_filter_update_streams(svo_b200_ctx* ctx, int S, co
     if (ftr_level[m] < 0 || ftr_level[m] >= ref_frames[ref_index[m]]->n_levels)
       return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: ftr_level[%d] outside the pyramid", m);
   }
+  // each stream's camera against its current frame and the keyframes its seeds refer to (the table is shared by streams
+  // of different cameras)
+  for (int s = 0; s < S; ++s) {
+    if (const int rc = cam_check_frames(ctx, "depth_filter_update_streams", cam + s, cur + s, 1)) return rc;
+    for (int m = seed_offset[s]; m < seed_offset[s + 1]; ++m)
+      if (const int rc = cam_check_frames(ctx, "depth_filter_update_streams", cam + s, ref_frames + ref_index[m], 1)) return rc;
+  }
   std::vector<DepthStream> st((size_t)S);
   for (int s = 0; s < S; ++s)
     if (const int rc = depth_stream(ctx, cur[s], cur_T_f_w + 12 * (size_t)s, cam + s, batch_counter[s], st[s])) return rc;
@@ -583,6 +592,8 @@ extern "C" int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_
   if (opt->max_search_level >= cur->n_levels)
     return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: max_search_level %d >= %d pyramid levels",
                    opt->max_search_level, cur->n_levels);
+  if (const int rc = cam_check_frames(ctx, "find_epipolar_match_direct", cam, &cur, 1)) return rc;
+  if (const int rc = cam_check_frames(ctx, "find_epipolar_match_direct", cam, ref_frames, n_ref)) return rc;
   DepthStream st;
   if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, 0, st)) return rc;
   const int seed_offset[2] = {0, M};

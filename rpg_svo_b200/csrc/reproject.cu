@@ -175,6 +175,8 @@ int reproject_check(svo_b200_ctx* ctx, const svo_b200_reproject_stream& a) {
     return set_err(ctx, SVO_B200_EINVAL, "reproject_map: NULL array in the map view");
   for (int k = 0; k < m->n_kfs; ++k)
     if (!kf_frames[k]) return set_err(ctx, SVO_B200_EINVAL, "reproject_map: kf_frames[%d] is NULL", k);
+  if (const int rc = cam_check_frames(ctx, "reproject_map", a.cam, &a.cur, 1)) return rc;
+  if (const int rc = cam_check_frames(ctx, "reproject_map", a.cam, kf_frames, m->n_kfs)) return rc;
   // the device and reproject_enumerate walk every [offset[i], offset[i+1]) range: each must lie inside the range
   // [0, offset[n]) whose entries are checked below
   for (int k = 0; k <= m->n_kfs && m->n_kfs > 0; ++k)

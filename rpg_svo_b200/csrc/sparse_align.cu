@@ -2481,6 +2481,7 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
         cur[b]->height != ref[0]->height || cur[b]->n_levels != ref[0]->n_levels)
       return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: all frames of a batch must share one geometry");
   }
+  if (int rc_sz = cam_check_frames(ctx, "sia_batch_stage", cam, ref, 1)) return rc_sz;  // ref[0]: the batch's one geometry
   if (st.total_feat > 0 && (!px || !f || !point_pos || !has_point))
     return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: NULL feature arrays");
   int rc = fill_common(ctx, st.P, ref[0], cam, opt);

@@ -22,6 +22,14 @@ def _same_bits(x, y):
 
 
 # ---- depth filter --------------------------------------------------------------------------------------------------------
+# one pixel narrower, shorter, wider, taller than the frames: refused (svo_b200_camera's size is its frames' level 0)
+SIZE_OFFSETS = [(-1, 0), (0, -1), (1, 0), (0, 1)]
+
+
+def _resized(cam, dw, dh):
+    return dataclasses.replace(cam, width=cam.width + dw, height=cam.height + dh)
+
+
 def _cam_644_radtan():
     return synth.Camera(330.0, 329.0, 321.5, 242.5, 644, 484, 0, (-0.28, 0.067, 0.0009, 0.0008, 0.0))
 
@@ -186,6 +194,8 @@ def test_depth_streams_refusals_write_nothing(ctx):
     x = base(); x["ri"] = np.array([0, 0, 0, -1, 0, 0, 0, 0], np.int32); bad.append(x)
     x = base(); x["lv"] = np.array([0, 0, 0, 0, 9, 0, 0, 0], np.int32); bad.append(x)              # level outside the pyramid
     x = base(); x["curs"] = (C.c_void_p * 2)(cur.h.value, small.h.value); bad.append(x)             # max_search_level 2 >= 2 levels
+    for dw, dh in SIZE_OFFSETS:                                                                    # a camera of another size
+        x = base(); x["cams"] = (capi.Camera * 2)(capi.cam_struct(c["cam"]), capi.cam_struct(_resized(c["cam"], dw, dh))); bad.append(x)
     for j, x in enumerate(bad):
         before = {k: v.copy() for k, v in x["seeds"].items()}
         n0 = ctx.launch_count()
@@ -204,6 +214,7 @@ def test_depth_streams_refusals_write_nothing(ctx):
     bad_cam = dataclasses.replace(c["cam"], model=7)
     singles = [dict(cur=None), dict(n_ref=0), dict(ri=np.array([0, 0, 0, 0, 0, 0, 0, 1], np.int32)),
                dict(lv=np.array([0, 0, 0, 0, 9, 0, 0, 0], np.int32)), dict(cur=small), dict(cam=bad_cam)]
+    singles += [dict(cam=_resized(c["cam"], dw, dh)) for dw, dh in SIZE_OFFSETS]
     for fn in ("update", "match"):
         for j, over in enumerate(singles + [dict(d_min=None)] * (fn == "match") + [dict(M=0, rc=0)]):
             x = dict(_raw_single_args(c, kf, cur, M), **over)
@@ -350,8 +361,9 @@ def test_reproject_streams_refusals_write_nothing(ctx):
     v = dict(cases[1]["view"]); v["pt_obs_offset"] = v["pt_obs_offset"].copy(); v["pt_obs_offset"][1] = v["pt_obs_offset"][-1] + 1000
     bads.append(dict(view=v))
     v = dict(cases[1]["view"]); v["kf_fts_offset"] = v["kf_fts_offset"].copy(); v["kf_fts_offset"][0] = -3; bads.append(dict(view=v))
+    bads += [dict(cam=_resized(cases[1]["cam"], dw, dh)) for dw, dh in SIZE_OFFSETS]                       # camera size != frames'
     # a single reproject_map call refused at the camera or cell-order check has already cleared its stats and actions
-    clears_single = (False, False, True, False, False, True, False, False)
+    clears_single = (False, False, True, False, False, True, False, False) + (False,) * len(SIZE_OFFSETS)
     for j, over in enumerate(bads):
         preps = []
         for i, c in enumerate(cases):
