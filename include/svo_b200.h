@@ -14,6 +14,7 @@
  *   svo_b200_find_epipolar_match_direct <- Matcher::findEpipolarMatchDirect   svo/include/svo/matcher.h:114-121
  *   svo_b200_depth_filter_update    <- DepthFilter::updateSeeds               svo/include/svo/depth_filter.h:155
  *                                      (Matcher::findEpipolarMatchDirect, updateSeed, computeTau inside)
+ *   svo_b200_set_epipolar_options   <- Matcher::Options of both               svo/include/svo/matcher.h:74-91
  *   (_streams: S streams' calls of reprojectMap / updateSeeds / FastDetector::detect in one launch each)
  *   svo_b200_frame_*                <- svo::Frame image pyramid               svo/include/svo/frame.h:52, svo/src/frame.cpp:156-165
  *   svo_b200_klt_*                  <- initialization::trackKlt's             svo/src/initialization.cpp:127-169
@@ -537,6 +538,28 @@ int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_b200_frame*
                                         double* depth_out, double* px_cur_out /*M*2*/, int* search_level_out,
                                         double* epi_length_out, uint8_t* reject_out, double* A_cur_ref_out /*M*4*/,
                                         int* n_zmssd_out);
+
+/* ---- Matcher::Options of the epipolar search (svo/include/svo/matcher.h:74-91, read by matcher.cpp:204-320) ----
+ * align_max_iter and max_epi_search_steps are the fields of svo_b200_depth_options; max_epi_length_optim is never read by
+ * the reference (matcher.cpp:226 uses the literal 2.0). */
+typedef struct {
+  int align_1d;                        /* Matcher::Options::align_1d (0): align1D along (px_A - px_B).cast<float>().normalized() */
+  int subpix_refinement;               /* (1): 0 = the scan's best step is the match, triangulated without alignment */
+  int epi_search_edgelet_filtering;    /* (1) */
+  double epi_search_edgelet_max_angle; /* (0.7): an edgelet is rejected when cosangle < max_angle (NaN never rejects) */
+} svo_b200_epipolar_options;
+/* Context setting like svo_b200_sia_robust.  NULL = the reference's defaults.  Applies to svo_b200_find_epipolar_match_direct,
+ * svo_b200_depth_filter_update and svo_b200_depth_filter_update_streams (all streams of a call).  At the defaults those
+ * run the kernel they always ran; any other setting runs its general instantiation, which follows each option as
+ * matcher.cpp does (the short-line branch, epi_length < 2, aligns whatever subpix_refinement says).  Any angle is
+ * accepted.  SVO_B200_EINVAL for a flag other than 0 or 1, and the setting is left as it was. */
+int svo_b200_set_epipolar_options(svo_b200_ctx* ctx, const svo_b200_epipolar_options* opt);
+int svo_b200_get_epipolar_options(const svo_b200_ctx* ctx, svo_b200_epipolar_options* out);
+/* Matcher::h_inv_ after each of the first M candidates of the last svo_b200_find_epipolar_match_direct call: ran_1d_out[m]
+ * is 1 when align1D ran for candidate m (it sets h_inv_ on entry, whether or not it converges) and h_inv_out[m] is the
+ * value it set; 0 and 0 when it did not run, and a Matcher's h_inv_ then keeps its previous value.  SVO_B200_EINVAL before
+ * the first such call, or when the last one had fewer than M candidates.  A refused call changes nothing. */
+int svo_b200_epipolar_last_h_inv(const svo_b200_ctx* ctx, int M, double* h_inv_out, uint8_t* ran_1d_out);
 
 /* ------------------------------------------------------------------ KLT tracking of the two-view initialisation ------ */
 /* initialization::trackKlt (svo/src/initialization.cpp:127-169) tracks every corner of the first keyframe into each new

@@ -66,6 +66,11 @@ class DepthOptions(C.Structure):
                 ("max_search_level", C.c_int), ("align_max_iter", C.c_int), ("max_epi_search_steps", C.c_int)]
 
 
+class EpipolarOptions(C.Structure):  # svo_b200_epipolar_options
+    _fields_ = [("align_1d", C.c_int), ("subpix_refinement", C.c_int), ("epi_search_edgelet_filtering", C.c_int),
+                ("epi_search_edgelet_max_angle", C.c_double)]
+
+
 SIA_STATS_DTYPE = np.dtype([("n_iters", np.int32), ("sum_visible", np.int32),
                             ("sum_in_image", np.int32), ("n_tracked", np.int32)])
 
@@ -357,6 +362,27 @@ class Context:
         out = np.zeros((int(B), MAX_LEVELS), np.float32)
         self._check(self.lib.svo_b200_sia_last_scales(self.h, int(B), _p(out)))
         return out
+
+    def set_epipolar_options(self, align_1d=False, subpix_refinement=True, edgelet_filtering=True, edgelet_max_angle=0.7):
+        """Matcher::Options of the epipolar search (svo_b200_set_epipolar_options) for find_epipolar_match_direct,
+        depth_filter_update and depth_filter_update_streams; the arguments' defaults are the reference's."""
+        o = EpipolarOptions(int(align_1d), int(subpix_refinement), int(edgelet_filtering), float(edgelet_max_angle))
+        self._check(self.lib.svo_b200_set_epipolar_options(self.h, C.byref(o)))
+
+    def epipolar_options(self) -> dict:
+        """The current setting (svo_b200_get_epipolar_options), in set_epipolar_options' keywords."""
+        o = EpipolarOptions()
+        self._check(self.lib.svo_b200_get_epipolar_options(self.h, C.byref(o)))
+        return dict(align_1d=bool(o.align_1d), subpix_refinement=bool(o.subpix_refinement),
+                    edgelet_filtering=bool(o.epi_search_edgelet_filtering), edgelet_max_angle=o.epi_search_edgelet_max_angle)
+
+    def epipolar_last_h_inv(self, M: int):
+        """(h_inv (M,) float64, ran_1d (M,) bool) of the first M candidates of the last find_epipolar_match_direct call
+        (svo_b200_epipolar_last_h_inv): ran_1d where align1D ran and set Matcher::h_inv_ to h_inv."""
+        h = np.zeros(max(int(M), 1))
+        r = np.zeros(max(int(M), 1), np.uint8)
+        self._check(self.lib.svo_b200_epipolar_last_h_inv(self.h, int(M), _p(h), _p(r)))
+        return h[:M], r[:M].astype(bool)
 
     def sia_batch_run(self):
         self._check(self.lib.svo_b200_sia_batch_run(self.h))

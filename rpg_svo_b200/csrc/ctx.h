@@ -95,6 +95,13 @@ struct svo_b200_ctx {
   // The last work enqueued on `stream` is a run of the staged batch (svo_b200_sia_batch_run): the next run of that batch
   // may then overlap it on the device.  Every other enqueue clears it (kt_begin for kernels; the copy-only entry points).
   bool sia_chain = false;
+  // svo_b200_set_epipolar_options: Matcher::Options of the depth filter / epipolar matcher launches
+  svo_b200_epipolar_options epi = {0, 1, 1, 0.7};
+  // per candidate of the last svo_b200_find_epipolar_match_direct call: Matcher::h_inv_ and whether align1D set it
+  // (svo_b200_epipolar_last_h_inv)
+  std::vector<double> epi_h_inv;
+  std::vector<uint8_t> epi_ran_1d;
+  bool epi_last_valid = false;
 };
 
 namespace svo {

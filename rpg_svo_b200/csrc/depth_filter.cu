@@ -58,6 +58,11 @@ struct DepthParams {
   double* epi_length_out;
   uint8_t* reject_out;
   double* A_out;
+  // Matcher::Options of svo_b200_set_epipolar_options, read only by the general instantiation; with match_only it also
+  // returns h_inv_ and whether align1D ran (svo_b200_epipolar_last_h_inv)
+  svo_b200_epipolar_options epi;
+  double* h_inv_out;
+  uint8_t* ran_1d_out;
 };
 
 // [EXT] vk::patch_score::ZMSSD<4>::computeScore on the 8x8 block whose top-left pixel is at byte
@@ -139,6 +144,9 @@ __device__ inline double compute_tau(const Pose& T_ref_cur, const double* f, dou
 // keyframe table shared by all streams.  The pose products (T_ref_cur, T_cur_ref) are formed per warp: a per-stream table
 // built on the host would round differently from the device's code, and one built on the device would cost a second
 // launch.  <= 128 registers: the 500 CTAs of C2 (2000 seeds) are resident at once.
+// kGeneral = false is Matcher::Options at its defaults (edgelet filter at 0.7, align2D, sub-pixel refinement); true reads
+// P.epi and follows every branch of matcher.cpp:204-212, 226-246 and 293-320 that the options select.
+template <bool kGeneral>
 __global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const DepthParams P,
                                                                          const DepthStream* __restrict__ streams,
                                                                          const int* __restrict__ seed_offset, int n_streams) {
@@ -206,12 +214,14 @@ __global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const De
     bool reject = false;
     int out_level = 0;
     double out_epi_length = 0.0;
-    if (P.ftr_type[i] == 1) {  // edgelet filtering (:204-212)
+    double h_inv = 0.0;
+    bool ran_1d = false;
+    if (P.ftr_type[i] == 1 && (!kGeneral || P.epi.epi_search_edgelet_filtering)) {  // edgelet filtering (:204-212)
       const double gx0 = P.ftr_grad[2 * i], gy0 = P.ftr_grad[2 * i + 1];
       const double gx = Aff[0] * gx0 + Aff[1] * gy0, gy = Aff[2] * gx0 + Aff[3] * gy0;
       const double gn = sqrt(gx * gx + gy * gy), en = sqrt(epi_x * epi_x + epi_y * epi_y);
       const double cosangle = fabs((gx / gn) * (epi_x / en) + (gy / gn) * (epi_y / en));
-      if (cosangle < 0.7) reject = true;
+      if (cosangle < (kGeneral ? P.epi.epi_search_edgelet_max_angle : 0.7)) reject = true;  // NaN on either side: kept
     }
     if (!reject) {
       const int L = best_search_level(Aff, P.max_search_level);
@@ -226,8 +236,8 @@ __global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const De
       warp_warp_affine(Aff, ref_img, pxu, pxv, lvl, L, S);
       ImgView cur_img = {st.cur.lvl[L], st.cur.w[L], st.cur.h[L]};
       const double sc = (double)(1 << L), inv_sc = 1.0 / sc;  // a power of two: x * inv_sc == x / sc exactly
-      bool have_start = false;
-      double start_u = 0, start_v = 0;
+      bool have_start = false, from_scan = false;
+      double start_u = 0, start_v = 0, uv_best_u = 0, uv_best_v = 0;
       if (epi_length < 2.0) {  // :226-246
         start_u = (pAu + pBu) * 0.5;
         start_v = (pAv + pBv) * 0.5;
@@ -276,15 +286,32 @@ __global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const De
           if (best_key < (long long)(2000 * 64) * 4294967296LL) {
             const int kb = (int)(best_key & 0xffffffffLL);
             const double ub = fma((double)kb, step_x, u0), vb = fma((double)kb, step_y, v0);
-            cam_world2cam(cam, ub, vb, start_u, start_v);  // px_cur_ = world2cam(uv_best)  (:299)
+            cam_world2cam(cam, ub, vb, start_u, start_v);  // px_cur_ = world2cam(uv_best)  (:297, :316)
             have_start = true;
+            if (kGeneral) { from_scan = true; uv_best_u = ub; uv_best_v = vb; }
           }
         }
       }
-      if (have_start) {  // subpixel refinement + triangulation (:295-315 / :229-245)
+      if (kGeneral && from_scan && !P.epi.subpix_refinement) {
+        // no refinement (:316-318): the scan's best step, triangulated along unproject2d(uv_best).normalized() with the
+        // squared norm summed and fused as the reference's build does ((u*u + v*v) + 1*1, two fused multiply-adds)
+        out_pu = start_u; out_pv = start_v;
+        const double n = sqrt(fma(1.0, 1.0, fma(uv_best_v, uv_best_v, uv_best_u * uv_best_u)));
+        const double f_cur[3] = {uv_best_u / n, uv_best_v / n, 1.0 / n};
+        ok = depth_from_triangulation(T_cur_ref, fv, f_cur, depth);
+      } else if (have_start) {  // subpixel refinement + triangulation (:295-315 / :229-245)
         double su = start_u / sc, sv = start_v / sc;
-        bool nan_exit = false;
-        const bool res = warp_align2d(cur_img, S, P.align_max_iter, su, sv, &nan_exit);
+        bool nan_exit = false, res;
+        if (kGeneral && P.epi.align_1d) {
+          // align1D along (px_A - px_B).cast<float>().normalized() (:231-234, :300-303): no guard on the norm, so a
+          // zero-length line gives a NaN direction, which align1D then runs with
+          const float dx = (float)ddx, dy = (float)ddy;
+          const float n = sqrtf(fmaf(dx, dx, __fmul_rn(dy, dy)));
+          res = warp_align1d(cur_img, S, __fdiv_rn(dx, n), __fdiv_rn(dy, n), P.align_max_iter, su, sv, h_inv, &nan_exit);
+          ran_1d = true;
+        } else {
+          res = warp_align2d(cur_img, S, P.align_max_iter, su, sv, &nan_exit);
+        }
         out_pu = start_u; out_pv = start_v;
         if (res) {
           out_pu = su * sc; out_pv = sv * sc;
@@ -300,6 +327,7 @@ __global__ void __launch_bounds__(kDfWarps * 32, 4) depth_filter_kernel(const De
         if (P.epi_length_out) P.epi_length_out[i] = out_epi_length;
         if (P.reject_out) P.reject_out[i] = reject ? 1 : 0;
         if (P.A_out) { P.A_out[4 * i] = Aff[0]; P.A_out[4 * i + 1] = Aff[1]; P.A_out[4 * i + 2] = Aff[2]; P.A_out[4 * i + 3] = Aff[3]; }
+        if (kGeneral) { P.h_inv_out[i] = h_inv; P.ran_1d_out[i] = ran_1d ? 1 : 0; }
       }
       status = ok ? SVO_B200_SEED_UPDATED : SVO_B200_SEED_NO_MATCH;
       out_z = ok ? depth : 0.0;
@@ -338,6 +366,11 @@ using namespace svo;
 
 namespace {
 
+// Matcher::Options() (svo/include/svo/matcher.h:83-91): the setting that runs the default instantiation
+bool epi_is_default(const svo_b200_epipolar_options& o) {
+  return !o.align_1d && o.subpix_refinement && o.epi_search_edgelet_filtering && o.epi_search_edgelet_max_angle == 0.7;
+}
+
 // The current frame, pose, camera and batch counter of one stream, as the kernel reads them.
 int depth_stream(svo_b200_ctx* ctx, const svo_b200_frame* cur, const double* cur_T_f_w, const svo_b200_camera* cam,
                  int batch_counter, DepthStream& st) {
@@ -356,6 +389,7 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
               int n_ref, const svo_b200_depth_options* opt, const DepthStream* streams, const int* seed_offset, int S) {
   const int M = H.M;
   const bool mo = H.match_only != 0;
+  const bool general = !epi_is_default(ctx->epi);
   cudaSetDevice(ctx->device);
   Carver c;
   const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),
@@ -373,9 +407,10 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
   const size_t in_bytes = c.off;
   const size_t o_st = c.take(M), o_pc = c.take(sizeof(double) * 2 * M), o_z = c.take(sizeof(double) * M),
                o_nz = c.take(sizeof(int) * M);
-  size_t o_sl = 0, o_el = 0, o_rj = 0, o_A = 0;
+  size_t o_sl = 0, o_el = 0, o_rj = 0, o_A = 0, o_hi = 0, o_r1 = 0;
   if (mo) {  // the Matcher's scratch members
     o_sl = c.take(sizeof(int) * M); o_el = c.take(sizeof(double) * M); o_rj = c.take(M); o_A = c.take(sizeof(double) * 4 * M);
+    if (general) { o_hi = c.take(sizeof(double) * M); o_r1 = c.take(M); }  // h_inv_ (align1D runs only here)
   }
   const size_t o_back = mo ? o_st : o_a;
   int rc;
@@ -437,6 +472,7 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
     P.epi_length_out = reinterpret_cast<double*>(d + o_el);
     P.reject_out = d + o_rj;
     P.A_out = reinterpret_cast<double*>(d + o_A);
+    if (general) { P.h_inv_out = reinterpret_cast<double*>(d + o_hi); P.ran_1d_out = d + o_r1; }
   } else {
     P.batch_id = reinterpret_cast<const int*>(d + o_bi);
     P.z_range = reinterpret_cast<float*>(d + o_zr);
@@ -446,9 +482,15 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
     P.sigma2 = reinterpret_cast<float*>(d + o_s2);
   }
   const int blocks = (M + kDfWarps - 1) / kDfWarps;
+  const DepthStream* d_streams = reinterpret_cast<const DepthStream*>(d + o_tab);
+  const int* d_seed_offset = reinterpret_cast<const int*>(d + o_so);
   kt_begin(ctx);
-  depth_filter_kernel<<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, reinterpret_cast<const DepthStream*>(d + o_tab),
-                                                                  reinterpret_cast<const int*>(d + o_so), S);
+  if (general) {
+    P.epi = ctx->epi;
+    depth_filter_kernel<true><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
+  } else {
+    depth_filter_kernel<false><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
+  }
   ctx->launches++;
   kt_end(ctx);
   SVO_CUDA_CHECK(ctx, cudaGetLastError());
@@ -460,6 +502,13 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
     if (H.epi_length_out) memcpy(H.epi_length_out, h + o_el, sizeof(double) * M);
     if (H.reject_out) memcpy(H.reject_out, h + o_rj, M);
     if (H.A_out) memcpy(H.A_out, h + o_A, sizeof(double) * 4 * M);
+    ctx->epi_h_inv.assign((size_t)M, 0.0);
+    ctx->epi_ran_1d.assign((size_t)M, 0);
+    if (general) {
+      memcpy(ctx->epi_h_inv.data(), h + o_hi, sizeof(double) * M);
+      memcpy(ctx->epi_ran_1d.data(), h + o_r1, M);
+    }
+    ctx->epi_last_valid = true;
   } else {
     memcpy(H.a, h + o_a, sizeof(float) * M);
     memcpy(H.b, h + o_b, sizeof(float) * M);
@@ -580,7 +629,10 @@ extern "C" int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_
                                                    int* n_zmssd_out) {
   if (!ctx || !ref_frames || !ref_T_f_w || n_ref <= 0 || !cur || !cur_T_f_w || !cam || !opt || M < 0)
     return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: bad arguments");
-  if (M == 0) return 0;
+  if (M == 0) {
+    ctx->epi_h_inv.clear(); ctx->epi_ran_1d.clear(); ctx->epi_last_valid = true;
+    return 0;
+  }
   if (!ref_index || !ftr_px || !ftr_f || !ftr_level || !ftr_type || !ftr_grad || !d_estimate || !d_min || !d_max || !success_out)
     return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: NULL candidate arrays");
   for (int m = 0; m < M; ++m) {
@@ -605,4 +657,34 @@ extern "C" int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_
   H.status = success_out; H.px_cur = px_cur_out; H.z = depth_out; H.n_zmssd = n_zmssd_out;
   H.search_level_out = search_level_out; H.epi_length_out = epi_length_out; H.reject_out = reject_out; H.A_out = A_cur_ref_out;
   return depth_run(ctx, H, ref_frames, ref_T_f_w, n_ref, opt, &st, seed_offset, 1);
+}
+
+extern "C" int svo_b200_set_epipolar_options(svo_b200_ctx* ctx, const svo_b200_epipolar_options* opt) {
+  if (!ctx) return SVO_B200_EINVAL;
+  if (!opt) {
+    ctx->epi = svo_b200_epipolar_options{0, 1, 1, 0.7};
+    return 0;
+  }
+  const auto flag = [](int v) { return v == 0 || v == 1; };
+  if (!flag(opt->align_1d) || !flag(opt->subpix_refinement) || !flag(opt->epi_search_edgelet_filtering))
+    return set_err(ctx, SVO_B200_EINVAL, "set_epipolar_options: flags must be 0 or 1 (align_1d %d, subpix_refinement %d, "
+                   "epi_search_edgelet_filtering %d)", opt->align_1d, opt->subpix_refinement, opt->epi_search_edgelet_filtering);
+  ctx->epi = *opt;
+  return 0;
+}
+
+extern "C" int svo_b200_get_epipolar_options(const svo_b200_ctx* ctx, svo_b200_epipolar_options* out) {
+  if (!ctx || !out) return SVO_B200_EINVAL;
+  *out = ctx->epi;
+  return 0;
+}
+
+extern "C" int svo_b200_epipolar_last_h_inv(const svo_b200_ctx* ctx, int M, double* h_inv_out, uint8_t* ran_1d_out) {
+  if (!ctx || M < 0 || !ctx->epi_last_valid || (size_t)M > ctx->epi_h_inv.size() || (M > 0 && (!h_inv_out || !ran_1d_out)))
+    return SVO_B200_EINVAL;
+  if (M > 0) {
+    memcpy(h_inv_out, ctx->epi_h_inv.data(), sizeof(double) * M);
+    memcpy(ran_1d_out, ctx->epi_ran_1d.data(), M);
+  }
+  return 0;
 }
