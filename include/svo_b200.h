@@ -582,8 +582,28 @@ void svo_b200_klt_pyramid_destroy(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr);
  * a pyramid is refused, not cut short, before anything is allocated or launched, and the handle keeps its last build. */
 int svo_b200_klt_pyramid_build(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr, const svo_b200_frame* frame, int max_level,
                                int with_derivatives);
-/* Number of levels the last build made (0 before the first). */
+/* Number of levels the last build made (0 before the first).  A build that fails to allocate a larger block
+ * (SVO_B200_ENOMEM) leaves the handle at 0 levels: svo_b200_klt_track refuses it until a build succeeds. */
 int svo_b200_klt_pyramid_levels(const svo_b200_klt_pyramid* pyr);
+
+/* The arguments of one svo_b200_klt_pyramid_build call, for svo_b200_klt_pyramid_build_streams. */
+typedef struct svo_b200_klt_build {
+  svo_b200_klt_pyramid* pyr;
+  const svo_b200_frame* frame;
+  int max_level;
+  int with_derivatives;
+} svo_b200_klt_build;
+/* S pyramids (e.g. the new frames of S camera streams) built together: one launch for level 0 of every entry, one pyrDown
+ * launch per level 1 .. L_max - 1 (L_max = the most levels any entry builds), and one Scharr launch over every level of
+ * every entry with derivatives -- the launch count depends on the deepest pyramid, not on S.  Entries may differ in size,
+ * max_level and with_derivatives; frame-pool frames are valid sources.  Every handle equals one svo_b200_klt_pyramid_build
+ * with its entry's arguments, byte for byte, and svo_b200_klt_pyramid_build is one entry of this call.  Every entry is
+ * checked as the single build checks it before anything is allocated, launched or written (SVO_B200_EINVAL, also for
+ * S < 0, NULL `builds` and a handle listed twice), so a refused call leaves every handle as it was.  SVO_B200_ELIMIT when
+ * a launch's tiles exceed one grid.  A failed allocation (SVO_B200_ENOMEM) returns before any launch; the handle it was
+ * for, and any handle already given a new block in the same call, is left at 0 levels.  S == 0 returns 0 without a
+ * launch. */
+int svo_b200_klt_pyramid_build_streams(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds);
 /* Copies one level out: img_out w*h bytes, deriv_out w*h*2 int16 (interleaved dx, dy; needs a build with derivatives);
  * either may be NULL. */
 int svo_b200_klt_pyramid_download(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* pyr, int level, uint8_t* img_out,
@@ -617,6 +637,28 @@ typedef struct {
 int svo_b200_klt_track(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* prev, const svo_b200_klt_pyramid* next,
                        const svo_b200_klt_options* opt, int N, const float* prev_pts, float* next_pts_io, uint8_t* status_out,
                        svo_b200_klt_exit* exit_out);
+
+/* The arguments of one svo_b200_klt_track call, for svo_b200_klt_track_streams. */
+typedef struct svo_b200_klt_stream {
+  const svo_b200_klt_pyramid* prev;
+  const svo_b200_klt_pyramid* next;
+  const svo_b200_klt_options* opt;
+  int N;
+  const float* prev_pts;
+  float* next_pts_io;
+  uint8_t* status_out;
+  svo_b200_klt_exit* exit_out; /* may be NULL */
+} svo_b200_klt_stream;
+/* S streams' calcOpticalFlowPyrLK (e.g. the initialisation of S camera streams that start together) in one launch: one
+ * copy to the device, one launch, one copy back, two stream synchronisations in all, as the single call makes.  Every
+ * stream's next_pts, statuses and exit records equal one svo_b200_klt_track call with that stream's arguments, bit for
+ * bit; svo_b200_klt_track is S = 1 of this call.  Streams may share pyramid handles (e.g. one first keyframe that several
+ * streams track against) and differ in image size and options; the output arrays of different streams must not overlap,
+ * while within one stream prev_pts and next_pts_io may be the same buffer.  Every stream's arguments are checked as
+ * svo_b200_klt_track checks them before anything is launched or written (SVO_B200_EINVAL, also for S < 0 or NULL
+ * `streams`), so a refused call leaves every output untouched.  SVO_B200_ELIMIT when the streams hold more than INT_MAX
+ * points together.  S == 0, or no points at all, returns 0 without a launch. */
+int svo_b200_klt_track_streams(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams);
 
 #ifdef __cplusplus
 }

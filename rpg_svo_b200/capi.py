@@ -107,6 +107,8 @@ def load() -> C.CDLL:
         _lib.svo_b200_klt_pyramid_download.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _lib.svo_b200_klt_track.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p]
+        _lib.svo_b200_klt_pyramid_build_streams.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.svo_b200_klt_track_streams.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     return _lib
 
 
@@ -821,26 +823,76 @@ def _klt_pyramid(self, frame: Frame, derivatives: bool, max_level: int = 4) -> K
     return KltPyramid(self).build(frame, derivatives, max_level)
 
 
-def _klt_track(self, prev: KltPyramid | None, nxt: KltPyramid | None, prev_pts, next_pts, max_level=4, max_iter=30, eps=0.001,
-               win_size=30, want_exit=True):
-    """calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, ..., OPTFLOW_USE_INITIAL_FLOW) on the device.
-    dict(next_pts (N x 2 float32), status (N uint8), and with want_exit: reason (N), level_reason / iters (N x MAX_LEVELS))."""
-    lib = self.lib
+class KltBuild(C.Structure):  # svo_b200_klt_build
+    _fields_ = [("pyr", C.c_void_p), ("frame", C.c_void_p), ("max_level", C.c_int), ("with_derivatives", C.c_int)]
+
+
+class KltStream(C.Structure):  # svo_b200_klt_stream
+    _fields_ = [("prev", C.c_void_p), ("next", C.c_void_p), ("opt", C.c_void_p), ("N", C.c_int), ("prev_pts", C.c_void_p),
+                ("next_pts_io", C.c_void_p), ("status_out", C.c_void_p), ("exit_out", C.c_void_p)]
+
+
+def _klt_prepare(prev: KltPyramid | None, nxt: KltPyramid | None, prev_pts, next_pts, max_level=4, max_iter=30, eps=0.001,
+                 win_size=30, want_exit=True):
+    """The svo_b200_klt_stream of one klt_track call, its outputs and the objects the call keeps alive."""
     p0 = np.ascontiguousarray(prev_pts, np.float32).reshape(-1, 2)
     p1 = np.ascontiguousarray(next_pts, np.float32).reshape(-1, 2).copy()
     n = len(p0)
     st = np.zeros(max(n, 1), np.uint8)
     ex = (KltExit * max(n, 1))() if want_exit else None
     opt = KltOptions(int(win_size), int(max_level), int(max_iter), float(eps))
-    self._check(lib.svo_b200_klt_track(self.h, prev.h if prev is not None else None, nxt.h if nxt is not None else None,
-                                       C.byref(opt), n, _p(p0), _p(p1), _p(st), ex))
-    o = dict(next_pts=p1, status=st[:n])
-    if want_exit:
-        o["reason"] = np.array([e.reason for e in ex[:n]], np.int32)
-        o["level_reason"] = np.array([list(e.level_reason) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
-        o["iters"] = np.array([list(e.iters) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
-    return o
+    ks = KltStream(prev.h.value if prev is not None else None, nxt.h.value if nxt is not None else None,
+                   C.cast(C.pointer(opt), C.c_void_p), n, p0.ctypes.data, p1.ctypes.data, st.ctypes.data,
+                   C.cast(ex, C.c_void_p) if ex is not None else None)
+    return ks, (p1, st, ex, n), (opt, p0)
+
+
+def _klt_result(o) -> dict:
+    p1, st, ex, n = o
+    r = dict(next_pts=p1, status=st[:n])
+    if ex is not None:
+        r["reason"] = np.array([e.reason for e in ex[:n]], np.int32)
+        r["level_reason"] = np.array([list(e.level_reason) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
+        r["iters"] = np.array([list(e.iters) for e in ex[:n]], np.int32).reshape(n, MAX_LEVELS)
+    return r
+
+
+def _klt_track(self, prev: KltPyramid | None, nxt: KltPyramid | None, prev_pts, next_pts, max_level=4, max_iter=30, eps=0.001,
+               win_size=30, want_exit=True):
+    """calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, ..., OPTFLOW_USE_INITIAL_FLOW) on the device.
+    dict(next_pts (N x 2 float32), status (N uint8), and with want_exit: reason (N), level_reason / iters (N x MAX_LEVELS))."""
+    ks, o, _keep = _klt_prepare(prev, nxt, prev_pts, next_pts, max_level, max_iter, eps, win_size, want_exit)
+    self._check(self.lib.svo_b200_klt_track(self.h, ks.prev, ks.next, ks.opt, ks.N, ks.prev_pts, ks.next_pts_io, ks.status_out,
+                                            ks.exit_out))
+    return _klt_result(o)
+
+
+def _klt_track_streams(self, streams):
+    """S streams' calcOpticalFlowPyrLK with one device launch (svo_b200_klt_track_streams).  `streams`: one dict per stream
+    with the arguments of klt_track by name (prev, nxt, prev_pts, next_pts and the optional max_level, max_iter, eps,
+    win_size, want_exit).  Returns one dict per stream, as klt_track returns."""
+    prep = [_klt_prepare(**s) for s in streams]
+    arr = (KltStream * max(len(prep), 1))(*[p[0] for p in prep])
+    self._check(self.lib.svo_b200_klt_track_streams(self.h, len(prep), arr))
+    return [_klt_result(o) for _, o, _ in prep]
+
+
+def _klt_pyramids(self, builds, pyramids=None):
+    """S LK pyramids built together (svo_b200_klt_pyramid_build_streams: one launch per stage, not per pyramid).  `builds`:
+    one dict per pyramid with frame, derivatives and the optional max_level (4); `pyramids`: handles to rebuild (one per
+    entry), new ones when None.  Returns the handles."""
+    pyrs = [KltPyramid(self) for _ in builds] if pyramids is None else list(pyramids)
+    assert len(pyrs) == len(builds)
+    arr = (KltBuild * max(len(builds), 1))(*[KltBuild(p.h.value if p.h else None, b["frame"].h.value if b["frame"].h else None,
+                                                      int(b.get("max_level", 4)), int(bool(b["derivatives"])))
+                                             for p, b in zip(pyrs, builds)])
+    self._check(self.lib.svo_b200_klt_pyramid_build_streams(self.h, len(builds), arr))
+    for p, b in zip(pyrs, builds):
+        p.width, p.height = b["frame"].width, b["frame"].height
+    return pyrs
 
 
 Context.klt_pyramid = _klt_pyramid
 Context.klt_track = _klt_track
+Context.klt_track_streams = _klt_track_streams
+Context.klt_pyramids = _klt_pyramids

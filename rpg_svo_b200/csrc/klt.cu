@@ -11,12 +11,17 @@
 //     partial in increasing pixel order followed by an xor-butterfly over the lanes: the order the oracle uses, so the
 //     kernel and the oracle agree bit for bit (-fmad=false keeps every product and sum rounded on its own, as OpenCV's
 //     scalar code does).  All lanes hold the same sums, so the per-point control flow is warp-uniform.
+//   * Many streams: one tracking launch and one pyramid build serve S streams (svo_b200_klt_track_streams,
+//     svo_b200_klt_pyramid_build_streams; DESIGN.md section 4.2e).  Each stream's levels, options and point offset sit in
+//     a table in global memory; a CTA finds its stream with stream_of.  The single calls are one stream of these.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 #include "ctx.h"
+#include "warp_align.cuh"
 
 struct svo_b200_klt_pyramid {
   int n_levels = 0, width = 0, height = 0;
@@ -44,21 +49,50 @@ __device__ __forceinline__ int reflect101(int p, int len) {  // cv::borderInterp
   return p;
 }
 
+// One image of a batched pyramid build launch (S pyramids' stage in one launch): CTA i of the launch is tile
+// i - cta_offset[j] of job j = stream_of(cta_offset, n_jobs, i), tiles of 32 x 8 pixels of the bordered level, row by row.
+//   level 0:  src = the frame's level 0 (pitch == w), dst = the bordered level 0
+//   pyrDown:  src = the bordered level above (sw wide), dst = the bordered level (w x h)
+//   Scharr:   src = the bordered level (w x h), der = its derivatives
+struct KltJob {
+  const uint8_t* src;
+  uint8_t* dst;
+  int* der;
+  int sw, w, h, tiles_x;
+};
+
+// the job of this CTA and the bordered pixel (X, Y) of this thread
+__device__ __forceinline__ const KltJob& klt_job(const KltJob* __restrict__ jobs, const int* __restrict__ cta_offset, int n_jobs,
+                                                 int& X, int& Y) {
+  const int j = stream_of(cta_offset, n_jobs, (int)blockIdx.x);
+  const KltJob& jb = jobs[j];
+  const int t = (int)blockIdx.x - __ldg(cta_offset + j);
+  const int ty = t / jb.tiles_x, tx = t - ty * jb.tiles_x;
+  X = tx * 32 + (int)threadIdx.x;
+  Y = ty * 8 + (int)threadIdx.y;
+  return jb;
+}
+
 // level 0 of the frame (pitch == width) into the bordered layout
-__global__ void klt_level0_kernel(const uint8_t* __restrict__ src, int w, int h, uint8_t* __restrict__ dst) {
+__global__ void __launch_bounds__(256) klt_level0_kernel(const KltJob* __restrict__ jobs, const int* __restrict__ cta_offset, int n_jobs) {
+  int X, Y;
+  const KltJob& jb = klt_job(jobs, cta_offset, n_jobs, X, Y);
+  const int w = jb.w, h = jb.h;
   const int S = w + 2 * kB, R = h + 2 * kB;
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= S || y >= R) return;
-  dst[(size_t)y * S + x] = src[(size_t)reflect101(y - kB, h) * w + reflect101(x - kB, w)];
+  if (X >= S || Y >= R) return;
+  jb.dst[(size_t)Y * S + X] = jb.src[(size_t)reflect101(Y - kB, h) * w + reflect101(X - kB, w)];
 }
 
 // pyrDown of the bordered level (sw, sh) into the bordered level (dw, dh): the border pixels are the filter's values at
 // their reflect-101 source, so the whole bordered level is written by one pass.  The source's 5 x 5 taps around
 // (2x, 2y) stay inside its border (2 pixels beyond the level at most) and read its reflect-101 continuation.
-__global__ void klt_down_kernel(const uint8_t* __restrict__ src, int sw, uint8_t* __restrict__ dst, int dw, int dh) {
-  const int S = dw + 2 * kB, R = dh + 2 * kB, SS = sw + 2 * kB;
-  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+__global__ void __launch_bounds__(256) klt_down_kernel(const KltJob* __restrict__ jobs, const int* __restrict__ cta_offset, int n_jobs) {
+  int X, Y;
+  const KltJob& jb = klt_job(jobs, cta_offset, n_jobs, X, Y);
+  const int dw = jb.w, dh = jb.h;
+  const int S = dw + 2 * kB, R = dh + 2 * kB, SS = jb.sw + 2 * kB;
   if (X >= S || Y >= R) return;
+  const uint8_t* __restrict__ src = jb.src;
   const int x = reflect101(X - kB, dw), y = reflect101(Y - kB, dh);
   const int k[5] = {1, 4, 6, 4, 1};
   int s = 0;
@@ -67,24 +101,26 @@ __global__ void klt_down_kernel(const uint8_t* __restrict__ src, int sw, uint8_t
     const uint8_t* row = src + (size_t)(2 * y + i - 2 + kB) * SS + (2 * x - 2 + kB);
     s += k[i] * (row[0] + 4 * row[1] + 6 * row[2] + 4 * row[3] + row[4]);
   }
-  dst[(size_t)Y * S + X] = (uint8_t)((s + 128) >> 8);
+  jb.dst[(size_t)Y * S + X] = (uint8_t)((s + 128) >> 8);
 }
 
 // Scharr derivatives of a bordered level: [3 10 3] x [-1 0 1], reflect-101 neighbours (the image's border), zero outside
 // the level.
-__global__ void klt_scharr_kernel(const uint8_t* __restrict__ img, int w, int h, int* __restrict__ der) {
+__global__ void __launch_bounds__(256) klt_scharr_kernel(const KltJob* __restrict__ jobs, const int* __restrict__ cta_offset, int n_jobs) {
+  int X, Y;
+  const KltJob& jb = klt_job(jobs, cta_offset, n_jobs, X, Y);
+  const int w = jb.w, h = jb.h;
   const int S = w + 2 * kB, R = h + 2 * kB;
-  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
   if (X >= S || Y >= R) return;
   int v = 0;
   if (X >= kB && X < kB + w && Y >= kB && Y < kB + h) {
-    const uint8_t* c = img + (size_t)Y * S + X;
+    const uint8_t* c = jb.src + (size_t)Y * S + X;
     const int t0m = (c[-S - 1] + c[S - 1]) * 3 + c[-1] * 10, t0p = (c[-S + 1] + c[S + 1]) * 3 + c[1] * 10;
     const int t1m = c[S - 1] - c[-S - 1], t1c = c[S] - c[-S], t1p = c[S + 1] - c[-S + 1];
     const int dx = t0p - t0m, dy = (t1p + t1m) * 3 + t1c * 10;
     v = (int)(uint16_t)(int16_t)dx | ((int)(int16_t)dy << 16);
   }
-  der[(size_t)Y * S + X] = v;
+  jb.der[(size_t)Y * S + X] = v;
 }
 
 struct KltLevels {
@@ -113,19 +149,20 @@ __device__ __forceinline__ bool out_of_bounds(float x, float y, int ix, int iy, 
   return ix < -kWin || ix >= w || iy < -kWin || iy >= h || isnan(x) || isnan(y);
 }
 
-__global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(KltLevels L, int max_iter, double eps2, int n,
-                                                               const float2* __restrict__ prev_pts, float2* __restrict__ next_pts,
-                                                               uint8_t* __restrict__ status, svo_b200_klt_exit* __restrict__ ex) {
-  __shared__ int16_t s_I[kWarps][kWinPx];
-  __shared__ int s_D[kWarps][kWinPx];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * kWarps + warp;
-  if (i >= n) return;
-  int16_t* sI = s_I[warp];
-  int* sD = s_D[warp];
+// One stream of a tracking launch: its levels (after the max_level cut), its clamped options, and where its points sit in
+// the launch's concatenated arrays (ex_off < 0: no exit records).
+struct KltStream {
+  KltLevels L;
+  double eps2;
+  int max_iter, n, pt_off, ex_off;
+};
+
+// One point, tracked by one warp: p0 = prevPts[ptidx], nxt = the initial guess nextPts[ptidx]; sI / sD the warp's window.
+// Lane 0 writes the point, its status and (ex non-null) its exit record.
+__device__ __forceinline__ void klt_track_point(const KltLevels& L, int max_iter, double eps2, float2 p0, float2 nxt, int lane,
+                                                int16_t* sI, int* sD, float2* next_out, uint8_t* status_out,
+                                                svo_b200_klt_exit* ex) {
   const float hw = (kWin - 1) * 0.5f;
-  const float2 p0 = prev_pts[i];
-  float2 nxt = next_pts[i];  // nextPts[ptidx]
   bool st = true;
   svo_b200_klt_exit e;
   e.reason = -1;
@@ -221,18 +258,318 @@ __global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(KltLevels L, int
     e.level_reason[level] = why;
   }
   if (lane == 0) {
-    next_pts[i] = nxt;
-    status[i] = st ? 1 : 0;
-    if (ex) { e.reason = e.level_reason[0]; ex[i] = e; }
+    *next_out = nxt;
+    *status_out = st ? 1 : 0;
+    if (ex) { e.reason = e.level_reason[0]; *ex = e; }
   }
 }
 
-inline dim3 grid2d(int S, int R) { return dim3((S + 31) / 32, (R + 7) / 8); }
+// One warp per point of n_streams streams' concatenated points: CTA i holds points (i - cta_offset[s]) * kWarps ... of
+// stream s = stream_of(cta_offset, n_streams, i) (stream s has ceil(n / kWarps) CTAs, so a CTA never spans two streams).
+// The initial guesses come in through `guess`, the results go out through next_pts.
+__global__ void __launch_bounds__(kWarps * 32) klt_track_kernel(const KltStream* __restrict__ streams, const int* __restrict__ cta_offset,
+                                                               int n_streams, const float2* __restrict__ prev_pts,
+                                                               const float2* __restrict__ guess, float2* __restrict__ next_pts,
+                                                               uint8_t* __restrict__ status, svo_b200_klt_exit* __restrict__ ex) {
+  __shared__ int16_t s_I[kWarps][kWinPx];
+  __shared__ int s_D[kWarps][kWinPx];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int s = stream_of(cta_offset, n_streams, (int)blockIdx.x);
+  const KltStream& st = streams[s];
+  const int k = ((int)blockIdx.x - __ldg(cta_offset + s)) * kWarps + warp;
+  if (k >= st.n) return;
+  const int i = st.pt_off + k;
+  klt_track_point(st.L, st.max_iter, st.eps2, prev_pts[i], guess[i], lane, s_I[warp], s_D[warp], next_pts + i, status + i,
+                  st.ex_off < 0 ? nullptr : ex + st.ex_off + k);
+}
+
+// S = 1: the same body with the stream's levels and options passed by value, from the parameter space.  A single stream's
+// launch is latency-bound (350 points at 752 x 480 are 88 CTAs), and there the table-driven launch measured about 7 %
+// slower (DESIGN.md section 4.2e).
+__global__ void __launch_bounds__(kWarps * 32) klt_track_one_kernel(const KltStream st, const float2* __restrict__ prev_pts,
+                                                                   const float2* __restrict__ guess, float2* __restrict__ next_pts,
+                                                                   uint8_t* __restrict__ status, svo_b200_klt_exit* __restrict__ ex) {
+  __shared__ int16_t s_I[kWarps][kWinPx];
+  __shared__ int s_D[kWarps][kWinPx];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * kWarps + warp;
+  if (i >= st.n) return;
+  klt_track_point(st.L, st.max_iter, st.eps2, prev_pts[i], guess[i], lane, s_I[warp], s_D[warp], next_pts + i, status + i,
+                  st.ex_off < 0 ? nullptr : ex + i);
+}
 
 }  // namespace
 }  // namespace svo
 
 using namespace svo;
+
+
+namespace {
+
+// The single build's argument checks and level cut (every entry's, for the batched build); nothing is written.
+int klt_build_check(svo_b200_ctx* ctx, const svo_b200_klt_build& b, int w[SVO_B200_MAX_LEVELS], int h[SVO_B200_MAX_LEVELS], int& n) {
+  const svo_b200_frame* frame = b.frame;
+  if (!ctx || !b.pyr || !frame || b.max_level < 0 || (b.with_derivatives != 0 && b.with_derivatives != 1))
+    return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: bad arguments");
+  n = 0;
+  for (int level = 0, cw = frame->width, ch = frame->height; level <= b.max_level; ++level) {
+    if (level == SVO_B200_MAX_LEVELS)  // OpenCV would build another level: refuse rather than track from a finer start
+      return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: %dx%d at max_level %d needs more than %d levels", frame->width,
+                     frame->height, b.max_level, SVO_B200_MAX_LEVELS);
+    w[level] = cw; h[level] = ch;  // buildOpticalFlowPyramid's level cut
+    n = level + 1;
+    cw = (cw + 1) / 2; ch = (ch + 1) / 2;
+    if (cw <= kWin || ch <= kWin) break;
+  }
+  return 0;
+}
+
+// One checked build entry: its level sizes and the offsets of its levels and derivatives in the handle's block.
+struct KltBuild {
+  int w[SVO_B200_MAX_LEVELS], h[SVO_B200_MAX_LEVELS], n = 0;
+  size_t off[SVO_B200_MAX_LEVELS], doff[SVO_B200_MAX_LEVELS], bytes = 0;
+};
+
+inline int tiles_x(int w) { return (w + 2 * kB + 31) / 32; }
+inline int64_t tiles(int w, int h) { return (int64_t)tiles_x(w) * ((h + 2 * kB + 7) / 8); }
+
+// A handle whose block is about to be freed: 0 levels, so that a track refuses it rather than read freed memory.
+void klt_unbuild(svo_b200_klt_pyramid* p) {
+  p->n_levels = 0;
+  p->width = p->height = 0;
+  p->derivs = false;
+  for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) { p->w[l] = p->h[l] = 0; p->img[l] = nullptr; p->der[l] = nullptr; }
+}
+
+// Every entry checked before anything is allocated or launched; then the handles that need a larger block get one (a
+// failed allocation returns before any launch, its handle left unbuilt); then one copy of the job tables to the device
+// and one launch per stage: level 0 of every entry, pyrDown of each level 1 .. L_max - 1 of every entry that has it, and
+// the Scharr derivatives of every level of every entry that asks for them.  The handles' levels are set last.
+int klt_build_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds, const char* name) {
+  std::vector<KltBuild> bs((size_t)S);
+  int L_max = 0;
+  bool any_der = false;
+  for (int s = 0; s < S; ++s) {
+    KltBuild& r = bs[s];
+    if (const int rc = klt_build_check(ctx, builds[s], r.w, r.h, r.n)) {
+      if (!ctx || name == nullptr) return rc;
+      const std::string why = ctx->err;
+      return set_err(ctx, rc, "%s: build %d: %s", name, s, why.c_str());
+    }
+    for (int t = 0; t < s; ++t)
+      if (builds[t].pyr == builds[s].pyr) return set_err(ctx, SVO_B200_EINVAL, "%s: builds %d and %d name one handle", name, t, s);
+    Carver c;
+    for (int l = 0; l < r.n; ++l) r.off[l] = c.take((size_t)(r.w[l] + 2 * kB) * (r.h[l] + 2 * kB));
+    for (int l = 0; l < r.n; ++l) r.doff[l] = builds[s].with_derivatives ? c.take((size_t)(r.w[l] + 2 * kB) * (r.h[l] + 2 * kB) * 4) : 0;
+    r.bytes = c.off;
+    L_max = std::max(L_max, r.n);
+    any_der = any_der || builds[s].with_derivatives;
+  }
+  // jobs of every launch, back to back: level 0, levels 1 .. L_max - 1, Scharr
+  const int n_launch = L_max + (any_der ? 1 : 0);
+  std::vector<int> n_jobs((size_t)n_launch, 0);
+  std::vector<int64_t> n_ctas((size_t)n_launch, 0);
+  for (int s = 0; s < S; ++s) {
+    const KltBuild& r = bs[s];
+    for (int l = 0; l < r.n; ++l) {
+      n_jobs[l]++;
+      n_ctas[l] += tiles(r.w[l], r.h[l]);
+      if (builds[s].with_derivatives) { n_jobs[L_max]++; n_ctas[L_max] += tiles(r.w[l], r.h[l]); }
+    }
+  }
+  for (int k = 0; k < n_launch; ++k)
+    if (n_ctas[k] > INT32_MAX)
+      return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld CTAs exceed one launch's grid", name ? name : "klt_pyramid_build",
+                     (long long)n_ctas[k]);
+  if (S == 0) return 0;
+  Carver c;
+  std::vector<size_t> o_jobs((size_t)n_launch), o_off((size_t)n_launch);
+  for (int k = 0; k < n_launch; ++k) {
+    o_jobs[k] = c.take(sizeof(KltJob) * n_jobs[k]);
+    o_off[k] = c.take(sizeof(int) * (n_jobs[k] + 1));
+  }
+  cudaSetDevice(ctx->device);
+  int rc;
+  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
+  for (int s = 0; s < S; ++s) {
+    svo_b200_klt_pyramid* p = builds[s].pyr;
+    if (bs[s].bytes <= p->bytes) continue;
+    klt_unbuild(p);
+    if (p->mem) {
+      void* old = p->mem;
+      p->mem = nullptr;
+      p->bytes = 0;
+      SVO_CUDA_CHECK(ctx, cudaFree(old));
+    }
+    if (cudaMalloc(&p->mem, bs[s].bytes) != cudaSuccess) {
+      cudaGetLastError();
+      p->mem = nullptr;
+      return set_err(ctx, SVO_B200_ENOMEM, "klt_pyramid_build: cudaMalloc(%zu) failed", bs[s].bytes);
+    }
+    p->bytes = bs[s].bytes;
+  }
+  std::vector<uint8_t> h(c.off);  // pageable: the copy stages it before returning, so no wait on earlier work
+  std::vector<int> fill((size_t)n_launch, 0);
+  for (int k = 0; k < n_launch; ++k) reinterpret_cast<int*>(h.data() + o_off[k])[0] = 0;
+  auto add = [&](int k, const KltJob& j) {
+    reinterpret_cast<KltJob*>(h.data() + o_jobs[k])[fill[k]] = j;
+    int* off = reinterpret_cast<int*>(h.data() + o_off[k]);
+    off[fill[k] + 1] = off[fill[k]] + (int)tiles(j.w, j.h);
+    fill[k]++;
+  };
+  for (int s = 0; s < S; ++s) {
+    const KltBuild& r = bs[s];
+    uint8_t* base = static_cast<uint8_t*>(builds[s].pyr->mem);
+    for (int l = 0; l < r.n; ++l) {
+      const uint8_t* src = l == 0 ? builds[s].frame->lvl(0) : base + r.off[l - 1];
+      add(l, KltJob{src, base + r.off[l], nullptr, l == 0 ? r.w[0] : r.w[l - 1], r.w[l], r.h[l], tiles_x(r.w[l])});
+      if (builds[s].with_derivatives)
+        add(L_max, KltJob{base + r.off[l], nullptr, reinterpret_cast<int*>(base + r.doff[l]), r.w[l], r.w[l], r.h[l], tiles_x(r.w[l])});
+    }
+  }
+  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
+  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h.data(), c.off, cudaMemcpyHostToDevice, ctx->stream));
+  kt_begin(ctx);
+  const dim3 blk(32, 8);
+  for (int k = 0; k < n_launch; ++k) {
+    const KltJob* jobs = reinterpret_cast<const KltJob*>(d + o_jobs[k]);
+    const int* off = reinterpret_cast<const int*>(d + o_off[k]);
+    if (k == 0) klt_level0_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+    else if (k < L_max) klt_down_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+    else klt_scharr_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+    ctx->launches++;
+  }
+  kt_end(ctx);
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  for (int s = 0; s < S; ++s) {
+    const KltBuild& r = bs[s];
+    svo_b200_klt_pyramid* p = builds[s].pyr;
+    uint8_t* base = static_cast<uint8_t*>(p->mem);
+    const bool der = builds[s].with_derivatives != 0;
+    p->n_levels = r.n;
+    p->width = builds[s].frame->width;
+    p->height = builds[s].frame->height;
+    p->derivs = der;
+    for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) {
+      p->w[l] = l < r.n ? r.w[l] : 0;
+      p->h[l] = l < r.n ? r.h[l] : 0;
+      p->img[l] = l < r.n ? base + r.off[l] : nullptr;
+      p->der[l] = l < r.n && der ? reinterpret_cast<int*>(base + r.doff[l]) : nullptr;
+    }
+  }
+  return 0;
+}
+
+// The single track's argument checks (every stream's, for the streams call); nothing is written.
+int klt_track_check(svo_b200_ctx* ctx, const svo_b200_klt_stream& a) {
+  const svo_b200_klt_pyramid *prev = a.prev, *next = a.next;
+  const svo_b200_klt_options* opt = a.opt;
+  if (!ctx || !prev || !next || !opt || a.N < 0) return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad arguments");
+  if (opt->win_size != kWin)
+    return set_err(ctx, SVO_B200_EINVAL, "klt_track: window size %d (only %d is supported)", opt->win_size, kWin);
+  if (opt->max_level < 0 || !(opt->eps >= 0.0))
+    return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad options (max_level %d, eps %g)", opt->max_level, opt->eps);
+  if (prev->n_levels == 0 || next->n_levels == 0 || !prev->derivs)
+    return set_err(ctx, SVO_B200_EINVAL, "klt_track: the previous pyramid needs a build with derivatives, the next one a build");
+  if (prev->width != next->width || prev->height != next->height)
+    return set_err(ctx, SVO_B200_EINVAL, "klt_track: images of different sizes (%dx%d, %dx%d)", prev->width, prev->height,
+                   next->width, next->height);
+  if (a.N > 0 && (!a.prev_pts || !a.next_pts_io || !a.status_out)) return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad arguments");
+  return 0;
+}
+
+// The table entry of one checked stream (point and exit offsets filled in by the caller).
+KltStream klt_stream_entry(const svo_b200_klt_stream& a) {
+  KltStream t;
+  std::memset(&t, 0, sizeof(t));
+  KltLevels& L = t.L;
+  L.n_levels = std::min(std::min(a.prev->n_levels, a.next->n_levels), a.opt->max_level + 1);
+  for (int l = 0; l < L.n_levels; ++l) {
+    L.I[l] = a.prev->img[l]; L.D[l] = a.prev->der[l]; L.J[l] = a.next->img[l];
+    L.w[l] = a.prev->w[l]; L.h[l] = a.prev->h[l];
+  }
+  t.max_iter = std::min(std::max(a.opt->max_iter, 0), 100);  // calcOpticalFlowPyrLK's clamps
+  const double eps = std::min(a.opt->eps, 10.0);
+  t.eps2 = eps * eps;
+  t.n = a.N;
+  return t;
+}
+
+// Every stream checked before anything is written; then one host-to-device copy (table, CTA offsets, every stream's
+// points and guesses), one launch, one copy back of every stream's points, statuses and exit records, and each stream's
+// share copied into its own outputs.
+int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, const char* name) {
+  std::vector<KltStream> tab((size_t)S);
+  int64_t n_pts = 0, n_ex = 0;
+  for (int s = 0; s < S; ++s) {
+    if (const int rc = klt_track_check(ctx, streams[s])) {
+      if (!ctx || name == nullptr) return rc;
+      const std::string why = ctx->err;
+      return set_err(ctx, rc, "%s: stream %d: %s", name, s, why.c_str());
+    }
+    tab[s] = klt_stream_entry(streams[s]);
+    tab[s].pt_off = (int)std::min<int64_t>(n_pts, INT32_MAX);
+    tab[s].ex_off = streams[s].exit_out ? (int)std::min<int64_t>(n_ex, INT32_MAX) : -1;
+    n_pts += streams[s].N;
+    if (streams[s].exit_out) n_ex += streams[s].N;
+  }
+  if (n_pts > INT32_MAX)
+    return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld points exceed one launch", name ? name : "klt_track", (long long)n_pts);
+  if (n_pts == 0) return 0;  // S == 0 included: no copy, no launch
+  const int N = (int)n_pts;
+  cudaSetDevice(ctx->device);
+  Carver ci, co;
+  const size_t i_tab = ci.take(sizeof(KltStream) * S), i_off = ci.take(sizeof(int) * (S + 1));
+  const size_t i_prev = ci.take((size_t)N * 8), i_guess = ci.take((size_t)N * 8);
+  const size_t o_next = co.take((size_t)N * 8), o_st = co.take((size_t)N), o_ex = co.take((size_t)n_ex * sizeof(svo_b200_klt_exit));
+  int rc;
+  if ((rc = ensure_host(ctx, ctx->h_in, ci.off)) || (rc = ensure_dev(ctx, ctx->d_in, ci.off)) ||
+      (rc = ensure_host(ctx, ctx->h_out, co.off)) || (rc = ensure_dev(ctx, ctx->d_out, co.off)))
+    return rc;
+  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  uint8_t* hi = static_cast<uint8_t*>(ctx->h_in.p);
+  uint8_t* di = static_cast<uint8_t*>(ctx->d_in.p);
+  uint8_t* ho = static_cast<uint8_t*>(ctx->h_out.p);
+  uint8_t* dout = static_cast<uint8_t*>(ctx->d_out.p);
+  int* off = reinterpret_cast<int*>(hi + i_off);
+  off[0] = 0;
+  for (int s = 0; s < S; ++s) {
+    const svo_b200_klt_stream& a = streams[s];
+    reinterpret_cast<KltStream*>(hi + i_tab)[s] = tab[s];
+    off[s + 1] = off[s] + (a.N + kWarps - 1) / kWarps;
+    if (a.N == 0) continue;
+    std::memcpy(hi + i_prev + (size_t)tab[s].pt_off * 8, a.prev_pts, (size_t)a.N * 8);
+    std::memcpy(hi + i_guess + (size_t)tab[s].pt_off * 8, a.next_pts_io, (size_t)a.N * 8);
+  }
+  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(di, hi, ci.off, cudaMemcpyHostToDevice, ctx->stream));
+  kt_begin(ctx);
+  const float2* d_prev = reinterpret_cast<const float2*>(di + i_prev);
+  const float2* d_guess = reinterpret_cast<const float2*>(di + i_guess);
+  float2* d_next = reinterpret_cast<float2*>(dout + o_next);
+  svo_b200_klt_exit* d_ex = reinterpret_cast<svo_b200_klt_exit*>(dout + o_ex);
+  if (S == 1)  // the table's entry by value (see klt_track_one_kernel); the staged table is then not read
+    klt_track_one_kernel<<<(unsigned)off[1], kWarps * 32, 0, ctx->stream>>>(tab[0], d_prev, d_guess, d_next, dout + o_st, d_ex);
+  else
+    klt_track_kernel<<<(unsigned)off[S], kWarps * 32, 0, ctx->stream>>>(reinterpret_cast<const KltStream*>(di + i_tab),
+                                                                         reinterpret_cast<const int*>(di + i_off), S, d_prev,
+                                                                         d_guess, d_next, dout + o_st, d_ex);
+  ctx->launches++;
+  kt_end(ctx);
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(ho, dout, co.off, cudaMemcpyDeviceToHost, ctx->stream));
+  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int s = 0; s < S; ++s) {
+    const svo_b200_klt_stream& a = streams[s];
+    if (a.N == 0) continue;
+    const size_t p = (size_t)tab[s].pt_off;
+    std::memcpy(a.next_pts_io, ho + o_next + p * 8, (size_t)a.N * 8);
+    std::memcpy(a.status_out, ho + o_st + p, (size_t)a.N);
+    if (a.exit_out) std::memcpy(a.exit_out, ho + o_ex + (size_t)tab[s].ex_off * sizeof(svo_b200_klt_exit), (size_t)a.N * sizeof(svo_b200_klt_exit));
+  }
+  return 0;
+}
+
+}  // namespace
 
 extern "C" int svo_b200_klt_pyramid_create(svo_b200_ctx* ctx, svo_b200_klt_pyramid** pyr_out) {
   if (!ctx || !pyr_out) return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_create: bad arguments");
@@ -253,60 +590,14 @@ extern "C" int svo_b200_klt_pyramid_levels(const svo_b200_klt_pyramid* pyr) { re
 
 extern "C" int svo_b200_klt_pyramid_build(svo_b200_ctx* ctx, svo_b200_klt_pyramid* pyr, const svo_b200_frame* frame, int max_level,
                                           int with_derivatives) {
-  if (!ctx || !pyr || !frame || max_level < 0 || (with_derivatives != 0 && with_derivatives != 1))
-    return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: bad arguments");
-  int w[SVO_B200_MAX_LEVELS], h[SVO_B200_MAX_LEVELS], n = 0;
-  for (int level = 0, cw = frame->width, ch = frame->height; level <= max_level; ++level) {
-    if (level == SVO_B200_MAX_LEVELS)  // OpenCV would build another level: refuse rather than track from a finer start
-      return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build: %dx%d at max_level %d needs more than %d levels", frame->width,
-                     frame->height, max_level, SVO_B200_MAX_LEVELS);
-    w[level] = cw; h[level] = ch;  // buildOpticalFlowPyramid's level cut
-    n = level + 1;
-    cw = (cw + 1) / 2; ch = (ch + 1) / 2;
-    if (cw <= kWin || ch <= kWin) break;
-  }
-  size_t off[SVO_B200_MAX_LEVELS], doff[SVO_B200_MAX_LEVELS];
-  Carver c;
-  for (int l = 0; l < n; ++l) off[l] = c.take((size_t)(w[l] + 2 * kB) * (h[l] + 2 * kB));
-  for (int l = 0; l < n; ++l) doff[l] = with_derivatives ? c.take((size_t)(w[l] + 2 * kB) * (h[l] + 2 * kB) * 4) : 0;
-  cudaSetDevice(ctx->device);
-  if (c.off > pyr->bytes) {
-    if (pyr->mem) SVO_CUDA_CHECK(ctx, cudaFree(pyr->mem));
-    pyr->mem = nullptr;
-    pyr->bytes = 0;
-    if (cudaMalloc(&pyr->mem, c.off) != cudaSuccess) {
-      cudaGetLastError();
-      return set_err(ctx, SVO_B200_ENOMEM, "klt_pyramid_build: cudaMalloc(%zu) failed", c.off);
-    }
-    pyr->bytes = c.off;
-  }
-  uint8_t* base = static_cast<uint8_t*>(pyr->mem);
-  pyr->n_levels = n;
-  pyr->width = frame->width;
-  pyr->height = frame->height;
-  pyr->derivs = with_derivatives != 0;
-  for (int l = 0; l < SVO_B200_MAX_LEVELS; ++l) {
-    pyr->w[l] = l < n ? w[l] : 0;
-    pyr->h[l] = l < n ? h[l] : 0;
-    pyr->img[l] = l < n ? base + off[l] : nullptr;
-    pyr->der[l] = l < n && with_derivatives ? reinterpret_cast<int*>(base + doff[l]) : nullptr;
-  }
-  kt_begin(ctx);
-  const dim3 blk(32, 8);
-  klt_level0_kernel<<<grid2d(w[0] + 2 * kB, h[0] + 2 * kB), blk, 0, ctx->stream>>>(frame->lvl(0), w[0], h[0], pyr->img[0]);
-  ctx->launches++;
-  for (int l = 1; l < n; ++l) {
-    klt_down_kernel<<<grid2d(w[l] + 2 * kB, h[l] + 2 * kB), blk, 0, ctx->stream>>>(pyr->img[l - 1], w[l - 1], pyr->img[l], w[l], h[l]);
-    ctx->launches++;
-  }
-  if (with_derivatives)
-    for (int l = 0; l < n; ++l) {
-      klt_scharr_kernel<<<grid2d(w[l] + 2 * kB, h[l] + 2 * kB), blk, 0, ctx->stream>>>(pyr->img[l], w[l], h[l], pyr->der[l]);
-      ctx->launches++;
-    }
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  return 0;
+  const svo_b200_klt_build b = {pyr, frame, max_level, with_derivatives};
+  return klt_build_run(ctx, 1, &b, nullptr);
+}
+
+extern "C" int svo_b200_klt_pyramid_build_streams(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds) {
+  if (!ctx || S < 0 || (S > 0 && !builds))
+    return set_err(ctx, SVO_B200_EINVAL, "klt_pyramid_build_streams: bad arguments (S %d)", S);
+  return klt_build_run(ctx, S, builds, "klt_pyramid_build_streams");
 }
 
 extern "C" int svo_b200_klt_pyramid_download(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* pyr, int level, uint8_t* img_out,
@@ -328,56 +619,12 @@ extern "C" int svo_b200_klt_pyramid_download(svo_b200_ctx* ctx, const svo_b200_k
 extern "C" int svo_b200_klt_track(svo_b200_ctx* ctx, const svo_b200_klt_pyramid* prev, const svo_b200_klt_pyramid* next,
                                   const svo_b200_klt_options* opt, int N, const float* prev_pts, float* next_pts_io,
                                   uint8_t* status_out, svo_b200_klt_exit* exit_out) {
-  if (!ctx || !prev || !next || !opt || N < 0) return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad arguments");
-  if (opt->win_size != kWin)
-    return set_err(ctx, SVO_B200_EINVAL, "klt_track: window size %d (only %d is supported)", opt->win_size, kWin);
-  if (opt->max_level < 0 || !(opt->eps >= 0.0))
-    return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad options (max_level %d, eps %g)", opt->max_level, opt->eps);
-  if (prev->n_levels == 0 || next->n_levels == 0 || !prev->derivs)
-    return set_err(ctx, SVO_B200_EINVAL, "klt_track: the previous pyramid needs a build with derivatives, the next one a build");
-  if (prev->width != next->width || prev->height != next->height)
-    return set_err(ctx, SVO_B200_EINVAL, "klt_track: images of different sizes (%dx%d, %dx%d)", prev->width, prev->height,
-                   next->width, next->height);
-  if (N == 0) return 0;
-  if (!prev_pts || !next_pts_io || !status_out) return set_err(ctx, SVO_B200_EINVAL, "klt_track: bad arguments");
-  KltLevels L;
-  std::memset(&L, 0, sizeof(L));
-  L.n_levels = std::min(std::min(prev->n_levels, next->n_levels), opt->max_level + 1);
-  for (int l = 0; l < L.n_levels; ++l) {
-    L.I[l] = prev->img[l]; L.D[l] = prev->der[l]; L.J[l] = next->img[l];
-    L.w[l] = prev->w[l]; L.h[l] = prev->h[l];
-  }
-  const int max_iter = std::min(std::max(opt->max_iter, 0), 100);  // calcOpticalFlowPyrLK's clamps
-  const double eps = std::min(opt->eps, 10.0);
-  cudaSetDevice(ctx->device);
-  Carver ci, co;
-  const size_t i_prev = ci.take((size_t)N * 8), i_next = ci.take((size_t)N * 8);
-  const size_t o_next = co.take((size_t)N * 8), o_st = co.take((size_t)N), o_ex = co.take(exit_out ? (size_t)N * sizeof(svo_b200_klt_exit) : 0);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, ci.off)) || (rc = ensure_dev(ctx, ctx->d_in, ci.off)) ||
-      (rc = ensure_host(ctx, ctx->h_out, co.off)) || (rc = ensure_dev(ctx, ctx->d_out, co.off)))
-    return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* hi = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* di = static_cast<uint8_t*>(ctx->d_in.p);
-  uint8_t* ho = static_cast<uint8_t*>(ctx->h_out.p);
-  uint8_t* dout = static_cast<uint8_t*>(ctx->d_out.p);
-  std::memcpy(hi + i_prev, prev_pts, (size_t)N * 8);
-  std::memcpy(hi + i_next, next_pts_io, (size_t)N * 8);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(di, hi, ci.off, cudaMemcpyHostToDevice, ctx->stream));
-  // the kernel reads the initial guess and writes the result through one array: the output slot starts as the guess
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(dout + o_next, di + i_next, (size_t)N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
-  kt_begin(ctx);
-  klt_track_kernel<<<(N + kWarps - 1) / kWarps, kWarps * 32, 0, ctx->stream>>>(
-      L, max_iter, eps * eps, N, reinterpret_cast<const float2*>(di + i_prev), reinterpret_cast<float2*>(dout + o_next), dout + o_st,
-      exit_out ? reinterpret_cast<svo_b200_klt_exit*>(dout + o_ex) : nullptr);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(ho, dout, co.off, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  std::memcpy(next_pts_io, ho + o_next, (size_t)N * 8);
-  std::memcpy(status_out, ho + o_st, (size_t)N);
-  if (exit_out) std::memcpy(exit_out, ho + o_ex, (size_t)N * sizeof(svo_b200_klt_exit));
-  return 0;
+  const svo_b200_klt_stream a = {prev, next, opt, N, prev_pts, next_pts_io, status_out, exit_out};
+  return klt_track_run(ctx, 1, &a, nullptr);
+}
+
+extern "C" int svo_b200_klt_track_streams(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams) {
+  if (!ctx || S < 0 || (S > 0 && !streams))
+    return set_err(ctx, SVO_B200_EINVAL, "klt_track_streams: bad arguments (S %d)", S);
+  return klt_track_run(ctx, S, streams, "klt_track_streams");
 }

@@ -11,8 +11,10 @@
 //       + static updateSeed/computeTau stay host-side in the reference and are not re-exported
 //                                                     svo/include/svo/depth_filter.h:101-158
 //   svo::Frame / Feature / Point / Seed               svo/include/svo/{frame,feature,point,depth_filter}.h
+//   svo::initialization::detectFeatures / trackKlt    svo/src/initialization.cpp:107-169
 //   svo::streams::updateSeeds / reprojectMap /        not in the reference: S objects' calls with one launch each;
-//     addKeyframes / detect / detectFeatures          updateSeeds / addKeyframes are for filters without a mapper thread
+//     addKeyframes / detect / detectFeatures /        updateSeeds / addKeyframes are for filters without a mapper thread;
+//     trackKlt                                        trackKlt builds the streams' LK pyramids with one batched build
 // The data model is the reference's pointer graph (std::list<Feature*>, Point*); the wrappers gather it
 // into the flat arrays the C ABI takes -- that gather is the cost SURVEY.md row a18 says must be
 // counted end to end.  Differences from the reference, all forced by the missing third-party types:
@@ -157,7 +159,7 @@ struct ATANCamera : AbstractCamera {  // vk::ATANCamera(width, height, fx, fy, c
 // One CUDA context per calling thread, as include/svo_b200.h asks.
 class Context {
  public:
-  explicit Context(int device = 0) {
+  explicit Context(int device = 0) : device_(device) {
     if (svo_b200_create(&ctx_, device) != 0)
       throw std::runtime_error("svo_b200_create failed: no usable CUDA device (there is no CPU fallback)");
   }
@@ -165,12 +167,14 @@ class Context {
   Context(const Context&) = delete;
   Context& operator=(const Context&) = delete;
   svo_b200_ctx* get() const { return ctx_; }
+  int device() const { return device_; }
   void check(int rc) const {
     if (rc != 0) throw std::runtime_error(std::string("svo_b200: ") + svo_b200_last_error(ctx_));
   }
 
  private:
   svo_b200_ctx* ctx_ = nullptr;
+  int device_ = 0;
 };
 
 class Frame;
@@ -253,14 +257,26 @@ class Frame {
   Context& context() const { return ctx_; }
   // The LK pyramid cv::calcOpticalFlowPyrLK builds from img_pyr_[0] (initialization::trackKlt), built on first use and
   // kept: the first keyframe's, with derivatives, serves every frame of the initialisation.
+  static constexpr int kKltMaxLevel = 4;  // calcOpticalFlowPyrLK's maxLevel in trackKlt (initialization.cpp:136)
   const svo_b200_klt_pyramid* kltPyramid(bool derivatives) {
-    if (!klt_) ctx_.check(svo_b200_klt_pyramid_create(ctx_.get(), &klt_));
-    if (klt_levels_ == 0 || (derivatives && !klt_derivs_)) {
-      ctx_.check(svo_b200_klt_pyramid_build(ctx_.get(), klt_, dev_, 4, derivatives ? 1 : 0));
-      klt_levels_ = svo_b200_klt_pyramid_levels(klt_);
-      klt_derivs_ = derivatives;
+    if (kltNeedsBuild(derivatives)) {
+      ctx_.check(svo_b200_klt_pyramid_build(ctx_.get(), kltHandle(), dev_, kKltMaxLevel, derivatives ? 1 : 0));
+      kltBuilt(true, derivatives);
     }
     return klt_;
+  }
+  // For builds of many frames' LK pyramids in one call (streams::trackKlt): whether kltPyramid(derivatives) would build,
+  // the handle such a build fills, and what the build did (ok = it succeeded; a failed one may have left the handle
+  // unbuilt, and the next use then builds again).
+  bool kltNeedsBuild(bool derivatives) const { return klt_levels_ == 0 || (derivatives && !klt_derivs_); }
+  svo_b200_klt_pyramid* kltHandle() {
+    if (!klt_) ctx_.check(svo_b200_klt_pyramid_create(ctx_.get(), &klt_));
+    return klt_;
+  }
+  void kltBuilt(bool ok, bool derivatives) {
+    klt_levels_ = svo_b200_klt_pyramid_levels(klt_);
+    if (ok) klt_derivs_ = derivatives;
+    else if (klt_levels_ == 0) klt_derivs_ = false;
   }
 
  private:
@@ -615,35 +631,109 @@ inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, 
   takeFeatures(new_features, px_vec, f_vec);
 }
 
+}  // namespace initialization
+
+// Many camera streams per GPU: S streams' initialization::trackKlt with one pyramid build and one tracking launch.
+namespace streams {
+
+// initialization::trackKlt(frames_ref[s], frames_cur[s], px_ref[s], px_cur[s], f_ref[s], f_cur[s], disparities[s]) of
+// every stream: every LK pyramid a frame does not yet hold is built in one batched build (svo_b200_klt_pyramid_build_streams;
+// the reference frames with derivatives, the current frames without, kept by the frames as Frame::kltPyramid keeps them),
+// all streams are tracked with one launch (svo_b200_klt_track_streams), and then, stream by stream, the lost points are
+// erased and f_cur (through the stream's own camera) and the disparities computed as the single function does.  Streams may
+// share frames (e.g. one first keyframe).  The device work runs on `ctx`, by default the context of frames_cur[0].  Vectors
+// of different lengths, a NULL frame, or a frame on another device than that context throw std::invalid_argument before
+// any object or vector changes.
+inline void trackKlt(const std::vector<FramePtr>& frames_ref, const std::vector<FramePtr>& frames_cur,
+                     std::vector<std::vector<Point2f>>& px_ref, std::vector<std::vector<Point2f>>& px_cur,
+                     std::vector<std::vector<Vector3d>>& f_ref, std::vector<std::vector<Vector3d>>& f_cur,
+                     std::vector<std::vector<double>>& disparities, Context* ctx = nullptr) {
+  const size_t S = frames_ref.size();
+  if (frames_cur.size() != S || px_ref.size() != S || px_cur.size() != S || f_ref.size() != S || f_cur.size() != S ||
+      disparities.size() != S)
+    throw std::invalid_argument("streams::trackKlt: one frame pair and one set of vectors per stream");
+  if (S == 0) return;
+  for (size_t s = 0; s < S; ++s)
+    if (!frames_ref[s] || !frames_cur[s]) throw std::invalid_argument("streams::trackKlt: NULL frame");
+  Context& c = ctx ? *ctx : frames_cur[0]->context();
+  for (size_t s = 0; s < S; ++s)
+    if (frames_ref[s]->context().device() != c.device() || frames_cur[s]->context().device() != c.device())
+      throw std::invalid_argument("streams::trackKlt: a frame lives on another device than the context");
+  // 1. the pyramids no frame holds yet, each frame once (with derivatives where any stream tracks from it)
+  std::vector<Frame*> todo;
+  std::vector<bool> der;
+  auto want = [&](Frame* f, bool d) {
+    if (!f->kltNeedsBuild(d)) return;
+    for (size_t k = 0; k < todo.size(); ++k)
+      if (todo[k] == f) { der[k] = der[k] || d; return; }
+    todo.push_back(f);
+    der.push_back(d);
+  };
+  for (size_t s = 0; s < S; ++s) { want(frames_ref[s].get(), true); want(frames_cur[s].get(), false); }
+  if (!todo.empty()) {
+    std::vector<svo_b200_klt_build> b(todo.size());
+    for (size_t k = 0; k < todo.size(); ++k) b[k] = {todo[k]->kltHandle(), todo[k]->device(), Frame::kKltMaxLevel, der[k] ? 1 : 0};
+    const int rc = svo_b200_klt_pyramid_build_streams(c.get(), (int)b.size(), b.data());
+    for (size_t k = 0; k < todo.size(); ++k) todo[k]->kltBuilt(rc == 0, der[k]);
+    c.check(rc);
+  }
+  // 2. one tracking launch: calcOpticalFlowPyrLK(ref, cur, px_ref, px_cur, ..., Size(30, 30), 4, (COUNT + EPS, 30, 0.001),
+  // OPTFLOW_USE_INITIAL_FLOW) of every stream
+  const svo_b200_klt_options opt = {30, Frame::kKltMaxLevel, 30, 0.001};
+  std::vector<std::vector<uint8_t>> status(S);
+  std::vector<svo_b200_klt_stream> a(S);
+  for (size_t s = 0; s < S; ++s) {
+    status[s].resize(px_ref[s].size());
+    px_cur[s].resize(px_ref[s].size());  // the reference requires the initial flow to have px_ref's size
+    a[s] = {frames_ref[s]->kltPyramid(true), frames_cur[s]->kltPyramid(false), &opt, (int)px_ref[s].size(),
+            reinterpret_cast<const float*>(px_ref[s].data()), reinterpret_cast<float*>(px_cur[s].data()), status[s].data(), nullptr};
+  }
+  c.check(svo_b200_klt_track_streams(c.get(), (int)S, a.data()));
+  // 3. per stream, in order: lost points erased from px_ref, px_cur and f_ref; f_cur and the disparities of the rest
+  // (initialization.cpp:146-168)
+  for (size_t s = 0; s < S; ++s) {
+    auto px_ref_it = px_ref[s].begin();
+    auto px_cur_it = px_cur[s].begin();
+    auto f_ref_it = f_ref[s].begin();
+    f_cur[s].clear(); f_cur[s].reserve(px_cur[s].size());
+    disparities[s].clear(); disparities[s].reserve(px_cur[s].size());
+    for (size_t i = 0; px_ref_it != px_ref[s].end(); ++i) {
+      if (!status[s][i]) {
+        px_ref_it = px_ref[s].erase(px_ref_it);
+        px_cur_it = px_cur[s].erase(px_cur_it);
+        f_ref_it = f_ref[s].erase(f_ref_it);
+        continue;
+      }
+      f_cur[s].push_back(frames_cur[s]->c2f(px_cur_it->x, px_cur_it->y));
+      const double dx = px_ref_it->x - px_cur_it->x, dy = px_ref_it->y - px_cur_it->y;  // float differences, widened
+      disparities[s].push_back(std::sqrt(dx * dx + dy * dy));
+      ++px_ref_it;
+      ++px_cur_it;
+      ++f_ref_it;
+    }
+  }
+}
+
+}  // namespace streams
+
+namespace initialization {
 // calcOpticalFlowPyrLK(ref, cur, px_ref, px_cur, ..., Size(30, 30), 4, (COUNT + EPS, 30, 0.001), OPTFLOW_USE_INITIAL_FLOW),
 // then lost points erased from px_ref, px_cur and f_ref in order; f_cur and the disparities of the rest (:127-169).
+// streams::trackKlt of one stream.
 inline void trackKlt(const FramePtr& frame_ref, const FramePtr& frame_cur, std::vector<Point2f>& px_ref, std::vector<Point2f>& px_cur,
                      std::vector<Vector3d>& f_ref, std::vector<Vector3d>& f_cur, std::vector<double>& disparities) {
-  const svo_b200_klt_options opt = {30, 4, 30, 0.001};
-  std::vector<uint8_t> status(px_ref.size());
-  px_cur.resize(px_ref.size());  // the reference requires the initial flow to have px_ref's size
-  Context& c = frame_cur->context();
-  c.check(svo_b200_klt_track(c.get(), frame_ref->kltPyramid(true), frame_cur->kltPyramid(false), &opt, (int)px_ref.size(),
-                             reinterpret_cast<const float*>(px_ref.data()), reinterpret_cast<float*>(px_cur.data()), status.data(), nullptr));
-  auto px_ref_it = px_ref.begin();
-  auto px_cur_it = px_cur.begin();
-  auto f_ref_it = f_ref.begin();
-  f_cur.clear(); f_cur.reserve(px_cur.size());
-  disparities.clear(); disparities.reserve(px_cur.size());
-  for (size_t i = 0; px_ref_it != px_ref.end(); ++i) {
-    if (!status[i]) {
-      px_ref_it = px_ref.erase(px_ref_it);
-      px_cur_it = px_cur.erase(px_cur_it);
-      f_ref_it = f_ref.erase(f_ref_it);
-      continue;
-    }
-    f_cur.push_back(frame_cur->c2f(px_cur_it->x, px_cur_it->y));
-    const double dx = px_ref_it->x - px_cur_it->x, dy = px_ref_it->y - px_cur_it->y;  // float differences, widened
-    disparities.push_back(std::sqrt(dx * dx + dy * dy));
-    ++px_ref_it;
-    ++px_cur_it;
-    ++f_ref_it;
+  std::vector<std::vector<Point2f>> pr(1), pc(1);
+  std::vector<std::vector<Vector3d>> fr(1), fc(1);
+  std::vector<std::vector<double>> d(1);
+  auto swap_all = [&] { pr[0].swap(px_ref); pc[0].swap(px_cur); fr[0].swap(f_ref); fc[0].swap(f_cur); d[0].swap(disparities); };
+  swap_all();
+  try {
+    streams::trackKlt({frame_ref}, {frame_cur}, pr, pc, fr, fc, d, frame_cur ? &frame_cur->context() : nullptr);
+  } catch (...) {
+    swap_all();
+    throw;
   }
+  swap_all();
 }
 }  // namespace initialization
 
