@@ -107,6 +107,22 @@ int svo_b200_set_pyramid_rule(svo_b200_ctx* ctx, int rule);
  * The copy is asynchronous on the context stream when host memory is pinned. */
 int svo_b200_frame_upload(svo_b200_ctx* ctx, svo_b200_frame* frame, const uint8_t* const* levels,
                           int n_given);
+/* The arguments of one single-level svo_b200_frame_upload call, for svo_b200_frame_upload_streams. */
+typedef struct svo_b200_frame_upload_entry {
+  svo_b200_frame* frame;  /* a frame of this context's device; frame-pool frames allowed */
+  const uint8_t* level0;  /* host image, pitch == frame width */
+} svo_b200_frame_upload_entry;
+/* S frames (e.g. the new frames of S camera streams) uploaded and their pyramids built together: each level 0 is copied
+ * straight into its frame, then one launch builds level 1 of every entry whose width is a multiple of 16 and that has more
+ * than one level, one launch makes the tiled copies no pyramid kernel makes, and one launch per fused pass (four levels
+ * each) serves every entry that needs the pass -- the launch count depends on the deepest pyramid, not on S: at most four
+ * for SVO_B200_MAX_LEVELS levels, two for 5-level frames whose widths are multiples of 16.  Entries may differ in size and
+ * level count, and may name frames of one pool, in any order.  Every frame's levels and tiled copies equal those of
+ * svo_b200_frame_upload(ctx, frame, &level0, 1), byte for byte, under either pyramid rule.  Every entry is checked before
+ * anything is copied, launched or written (SVO_B200_EINVAL for S < 0, NULL `entries`, a NULL frame or image and a frame
+ * listed twice), so a refused call leaves every frame as it was.  SVO_B200_ELIMIT when a launch's work exceeds one grid.
+ * S == 0 returns 0 without a launch.  The copies are asynchronous on the context stream when the host memory is pinned. */
+int svo_b200_frame_upload_streams(svo_b200_ctx* ctx, int S, const svo_b200_frame_upload_entry* entries);
 /* Device-to-device variant: level 0 already on this GPU. */
 int svo_b200_frame_upload_device(svo_b200_ctx* ctx, svo_b200_frame* frame, const void* level0_dev);
 int svo_b200_frame_download_level(svo_b200_ctx* ctx, const svo_b200_frame* frame, int level,

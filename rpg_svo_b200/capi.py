@@ -109,6 +109,7 @@ def load() -> C.CDLL:
                                             C.c_void_p, C.c_void_p]
         _lib.svo_b200_klt_pyramid_build_streams.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _lib.svo_b200_klt_track_streams.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.svo_b200_frame_upload_streams.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     return _lib
 
 
@@ -892,6 +893,30 @@ def _klt_pyramids(self, builds, pyramids=None):
     return pyrs
 
 
+class FrameUploadEntry(C.Structure):  # svo_b200_frame_upload_entry
+    _fields_ = [("frame", C.c_void_p), ("level0", C.c_void_p)]
+
+
+def _frames_upload(self, entries):
+    """S frames' level-0 uploads and pyramid builds together (svo_b200_frame_upload_streams: one launch per stage, not per
+    frame); each frame ends as Frame.upload([image]) leaves it.  `entries`: (frame, image) pairs, the image a uint8 array of
+    the frame's size, or the address of one in pinned host memory that the caller keeps alive.  The call waits for the
+    device only when an entry is an array.  Returns the frames."""
+    keep, arr = [], (FrameUploadEntry * max(len(entries), 1))()
+    for i, (f, im) in enumerate(entries):
+        if not isinstance(im, int):
+            im = np.ascontiguousarray(im, dtype=np.uint8)
+            assert im.shape == (f.height, f.width), (im.shape, i)
+            keep.append(im)
+            im = im.ctypes.data
+        arr[i] = FrameUploadEntry(f.h.value if f.h else None, im)
+    self._check(self.lib.svo_b200_frame_upload_streams(self.h, len(entries), arr))
+    if keep:
+        self.synchronize()  # host arrays may be freed by the caller right after
+    return [f for f, _ in entries]
+
+
+Context.frames_upload = _frames_upload
 Context.klt_pyramid = _klt_pyramid
 Context.klt_track = _klt_track
 Context.klt_track_streams = _klt_track_streams

@@ -234,6 +234,12 @@ class Frame {
     ctx_.check(svo_b200_synchronize(ctx_.get()));
     for (int l = 0; l < n_levels; ++l) img_pyr_.push_back(Image{this, l, cam->width_ >> l, cam->height_ >> l});
   }
+  // A frame whose device pyramid is allocated but not yet uploaded: streams::newFrames uploads many with one call.
+  struct NotUploaded {};
+  Frame(Context& ctx, AbstractCamera* cam, int n_levels, NotUploaded) : cam_(cam), ctx_(ctx) {
+    ctx_.check(svo_b200_frame_create(ctx_.get(), cam->width_, cam->height_, n_levels, &dev_));
+    for (int l = 0; l < n_levels; ++l) img_pyr_.push_back(Image{this, l, cam->width_ >> l, cam->height_ >> l});
+  }
   ~Frame() {
     for (Feature* f : fts_) delete f;  // frame.cpp:43-46
     svo_b200_klt_pyramid_destroy(ctx_.get(), klt_);
@@ -633,8 +639,33 @@ inline void detectFeatures(const FramePtr& frame, std::vector<Point2f>& px_vec, 
 
 }  // namespace initialization
 
-// Many camera streams per GPU: S streams' initialization::trackKlt with one pyramid build and one tracking launch.
+// Many camera streams per GPU: S streams' new frames with one batched upload, and S streams' initialization::trackKlt with one
+// pyramid build and one tracking launch.
 namespace streams {
+
+// new Frame(ctx, cams[s], imgs[s], n_levels, timestamps[s]) of every stream: S frames whose device pyramids equal the
+// constructor's, uploaded and built with one svo_b200_frame_upload_streams call and one synchronisation for all S.  Vectors
+// of different lengths and a NULL camera throw std::invalid_argument, a NULL image throws as the constructor does
+// (frame.cpp:51-52), before any frame is created.
+inline std::vector<FramePtr> newFrames(Context& ctx, const std::vector<AbstractCamera*>& cams, const std::vector<const uint8_t*>& imgs,
+                                       int n_levels, const std::vector<double>& timestamps) {
+  const size_t S = cams.size();
+  if (imgs.size() != S || timestamps.size() != S)
+    throw std::invalid_argument("streams::newFrames: one camera, image and timestamp per stream");
+  for (size_t s = 0; s < S; ++s) {
+    if (!cams[s]) throw std::invalid_argument("streams::newFrames: NULL camera");
+    if (!imgs[s]) throw std::runtime_error("Frame: provided image is empty");
+  }
+  std::vector<FramePtr> frames;
+  std::vector<svo_b200_frame_upload_entry> e(S);
+  for (size_t s = 0; s < S; ++s) {
+    frames.emplace_back(new Frame(ctx, cams[s], n_levels, Frame::NotUploaded{}));
+    e[s] = {frames[s]->device(), imgs[s]};
+  }
+  ctx.check(svo_b200_frame_upload_streams(ctx.get(), (int)S, e.data()));  // createImgPyramid of every frame on the device
+  ctx.check(svo_b200_synchronize(ctx.get()));
+  return frames;
+}
 
 // initialization::trackKlt(frames_ref[s], frames_cur[s], px_ref[s], px_cur[s], f_ref[s], f_cur[s], disparities[s]) of
 // every stream: every LK pyramid a frame does not yet hold is built in one batched build (svo_b200_klt_pyramid_build_streams;

@@ -8,7 +8,8 @@ four maps of that shape (seeds 4001..4004).  FAST detector: the keyframe seeding
 streams cycle through four such keyframes.  KLT: one step of the two-view initialisation per stream (scripts/bench_klt.py's
 workload: a 752x480 pair, 350 points, window 30, max_level 4), the new frame's LK pyramid build plus the tracking, against
 a reference pyramid built once per stream; single = one pyramid build and one track call per stream, batched = one
-svo_b200_klt_pyramid_build_streams and one svo_b200_klt_track_streams call; the streams cycle through four pairs.  For
+svo_b200_klt_pyramid_build_streams and one svo_b200_klt_track_streams call; the streams cycle through four pairs.  Frames:
+each stream's new frame (bench_frames), device and wall time as medians.  For
 S = 1, 8, 32, 132 it times,
 with CUDA events on the context's stream around the whole host call (staging, launch(es), copies back and, for the
 reprojector and the detector, the host replay or decode), S back-to-back single calls and one batched call, alternating them; it reports the medians
@@ -16,7 +17,7 @@ of --reps runs after --warmup runs of each, the kernel-only time of the batched 
 build's launches plus the tracking launch, from a run of their own), and
 checks that both produce the same bits.  Prints one JSON line per (stage, S) and the card it ran on.
 
-    python scripts/bench_streams.py [--reps 50] [--warmup 5] [--streams 1,8,32,132] [--stages depth_filter,reprojector,fast_detect,klt]
+    python scripts/bench_streams.py [--reps 50] [--warmup 5] [--streams 1,8,32,132] [--stages depth_filter,reprojector,fast_detect,klt,frames]
 """
 from __future__ import annotations
 
@@ -74,13 +75,89 @@ def bench(ctx, name, single, batched, same, reps, warmup, S, kernel=None):
     return r
 
 
+def _frame_states(frames):
+    return [(f.download_level(l).tobytes(), f.download_level_tiled(l).tobytes()) for f in frames for l in range(f.n_levels)]
+
+
+def _timed_pair(ctx, fn):
+    """(device ms from CUDA events around fn, wall ms from before fn to after a synchronise)."""
+    import time
+
+    import torch
+
+    s = torch.cuda.ExternalStream(ctx.stream)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0 = time.perf_counter()
+    e0.record(s)
+    fn()
+    e1.record(s)
+    ctx.synchronize()
+    t1 = time.perf_counter()
+    return e0.elapsed_time(e1), 1e3 * (t1 - t0)
+
+
+def _frames_leg(ctx, name, single, batched, S, reps, warmup, extra):
+    for _ in range(warmup):
+        single(); batched()
+    ds, ws, db, wb, ks, kb = [], [], [], [], [], []
+    for _ in range(reps):
+        d, w = _timed_pair(ctx, single)
+        ds.append(d); ws.append(w); ks.append(ctx.last_kernel_ms())
+        d, w = _timed_pair(ctx, batched)
+        db.append(d); wb.append(w); kb.append(ctx.last_kernel_ms())
+    med = lambda x: float(np.median(x))  # noqa: E731
+    r = dict(stage=name, S=S, single_device_ms=med(ds), single_wall_ms=med(ws), batched_device_ms=med(db), batched_wall_ms=med(wb),
+             single_last_kernel_ms=med(ks), batched_kernel_ms=med(kb), device_speedup=med(ds) / med(db),
+             wall_speedup=med(ws) / med(wb), reps=reps, **extra)
+    print(json.dumps(r), flush=True)
+    return r
+
+
+def bench_frames(ctx, Ss, reps, warmup):
+    """S single svo_b200_frame_upload calls against one svo_b200_frame_upload_streams call: one 5-level frame per stream (what
+    FrameHandlerMono builds: max(n_pyr_levels, klt_max_level + 1)), sizes cycling through 752x480, 640x480 and 644x484, level
+    0 from pinned host buffers.  single_last_kernel_ms is the last single call's kernels (its S = 1 value is one upload).  Then
+    one 64-frame window of a 7-level 752x480 pool: one svo_b200_frame_pool_upload against one batched call over its 64 frames."""
+    import torch
+
+    sizes = [(752, 480), (640, 480), (644, 484)]
+    out = []
+    for S in Ss:
+        shapes = [sizes[s % 3] for s in range(S)]
+        host = [torch.from_numpy(np.random.default_rng(900 + s).integers(0, 256, (h, w), dtype=np.uint8)).pin_memory()
+                for s, (w, h) in enumerate(shapes)]
+        fs = [capi.Frame(ctx, w, h, 5) for w, h in shapes]
+        fb = [capi.Frame(ctx, w, h, 5) for w, h in shapes]
+
+        def single(fs=fs, host=host):
+            for f, im in zip(fs, host):
+                f.upload_ptrs([im.data_ptr()])
+
+        def batched(fb=fb, host=host):
+            ctx.frames_upload([(f, im.data_ptr()) for f, im in zip(fb, host)])
+
+        out.append(_frames_leg(ctx, "frames", single, batched, S, reps, warmup, {}))
+        assert _frame_states(fs) == _frame_states(fb), f"frames S={S}: batched pyramids differ from single uploads"
+        for f in fs + fb:
+            f.destroy()
+    pool_s, pool_b = capi.FramePool(ctx, 752, 480, 7, 64), capi.FramePool(ctx, 752, 480, 7, 64)
+    host = torch.from_numpy(np.random.default_rng(964).integers(0, 256, (64, 480, 752), dtype=np.uint8)).pin_memory()
+    ptrs = [host[i].data_ptr() for i in range(64)]
+    out.append(_frames_leg(ctx, "frames_pool_window", lambda: pool_s.upload(0, 64, host.data_ptr(), 752 * 480),
+                           lambda: ctx.frames_upload(list(zip(pool_b.frames, ptrs))), 64, reps, warmup,
+                           dict(note="single = one frame_pool_upload of a 64-frame 7-level 752x480 window")))
+    assert _frame_states(pool_s.frames) == _frame_states(pool_b.frames), "pool window: batched pyramids differ"
+    pool_s.destroy(); pool_b.destroy()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--streams", default="1,8,32,132")
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
-    ap.add_argument("--stages", default="depth_filter,reprojector,fast_detect,klt")
+    ap.add_argument("--stages", default="depth_filter,reprojector,fast_detect,klt,frames")
     a = ap.parse_args()
     Ss = [int(x) for x in a.streams.split(",")]
     stages = a.stages.split(",")
@@ -201,6 +278,9 @@ def main():
             results.append(bench(ctx, "klt", single, batched, same, a.reps, a.warmup, S, kernel))
             for pc in own:
                 pc.destroy()
+    # ---- frames: every stream's new frame, level 0 from pinned host memory, pyramid on the device ----
+    if "frames" in stages:
+        results += bench_frames(ctx, Ss, a.reps, a.warmup)
     if a.out:
         with open(a.out, "w") as f:
             for r in results:
