@@ -43,6 +43,7 @@
 #include <vector>
 
 #include "ctx.h"
+#include "sia_patch_layout.h"
 #include "svo_math.cuh"
 
 namespace svo {
@@ -792,7 +793,7 @@ struct SiaInst {
   // dynamic shared memory: control block (SH, then UPT when UP), patch array sets, xyz_ref (SS), staging region
   static constexpr size_t kShBytes = (sizeof(SH) + 15) & ~size_t(15);
   static constexpr size_t kCtlBytes = kShBytes + (UP ? ((sizeof(UPT) + 15) & ~size_t(15)) : 0);
-  static constexpr size_t kSetFloats = (size_t)3 * kPatchArea * SA;  // one set: [16][SA] f32 patch, [16][SA] float2 gradients
+  static constexpr size_t kSetFloats = (size_t)3 * kPatchArea * SA;  // one set: SA slots of patch and gradients (sia_patch_chunk)
   static constexpr size_t kXyzDoubles = SS ? (size_t)3 * SA : 0;     // [3][SA] f64 xyz_ref
   // bytes in front of the staging region with n_sets patch array sets (1, or one per level when UP)
   static constexpr size_t fixed_bytes(int n_sets) {
@@ -832,11 +833,10 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   // the regions in the order of SiaInst::fixed_bytes (pointer steps in the regions' element types: stepping in bytes
   // instead changes the generated address arithmetic)
   float* const pat_base = reinterpret_cast<float*>(smem_raw + G::kCtlBytes);
-  // set li (0 = coarsest level) : [16][SA] f32 reference patch, then [16][SA] float2 gradients
-  auto pat_ref_of = [&](int li) -> float* { return pat_base + (size_t)li * G::kSetFloats; };
-  auto pat_dxy_of = [&](int li) -> float2* { return reinterpret_cast<float2*>(pat_ref_of(li) + kPatchArea * SA); };
-  float* pat_ref = pat_ref_of(0);
-  float2* pat_dxy = pat_dxy_of(0);
+  // set li (0 = coarsest level): each slot's reference patch and gradients as 16-byte chunks, addressed by sia_patch_chunk
+  auto pat_of = [&](int li) -> uint8_t* { return reinterpret_cast<uint8_t*>(pat_base + (size_t)li * G::kSetFloats); };
+  auto pchunk = [&](uint8_t* set, int slot, int c) -> float4* { return reinterpret_cast<float4*>(set + sia_patch_chunk(SA, slot, c)); };
+  uint8_t* pat = pat_of(0);
   double* const st_xyz = reinterpret_cast<double*>(pat_base + (size_t)n_lvl_bufs * G::kSetFloats);  // SS: [3][SA] xyz_ref
   uint8_t* stage = reinterpret_cast<uint8_t*>(st_xyz + G::kXyzDoubles);  // 16-byte aligned
   uint4* win = reinterpret_cast<uint4*>(stage);                                                      // [kWinRows][SA] 16-byte window rows
@@ -870,7 +870,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     if (np_loc > 0) {
       const uint32_t bytes = (uint32_t)np_loc * 65u;
       mbar_expect_tx(&s.mbar, bytes);
-      uint8_t* dst = reinterpret_cast<uint8_t*>(pat_ref);
+      uint8_t* dst = pat;
       const uint8_t* src = job.blob;
       tma_bulk_g2s(dst, src + (size_t)fbase * 16, (uint32_t)np_loc * 16u, &s.mbar);                                   // px
       tma_bulk_g2s(dst + (size_t)np_loc * 16, src + (size_t)np * 16 + (size_t)fbase * 24, (uint32_t)np_loc * 24u, &s.mbar);  // f
@@ -897,7 +897,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
   }
   __syncthreads();
   mbar_wait(&s.mbar, 0);
-  const uint8_t* blob = reinterpret_cast<const uint8_t*>(pat_ref);
+  const uint8_t* blob = pat;
   const double* b_f = reinterpret_cast<const double*>(blob) + 2 * np_loc;
   const double* b_pos = b_f + 3 * np_loc;
   const uint8_t* b_hp = reinterpret_cast<const uint8_t*>(b_pos + 3 * np_loc);
@@ -1042,33 +1042,36 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     }
   };
   // ---- gradient moments Sxx, Sxy, Syy of feature k of this thread if it is in `mask` (else zero), summed pixel by pixel
-  //      from the gradient array pd in shared memory; patch_moments: of all its features
-  auto feat_moments = [&](const float2* pd, const unsigned mask, const int k, double& sxx, double& sxy, double& syy) {
+  //      from the gradients of patch array set `set` in shared memory; patch_moments: of all its features
+  auto feat_moments = [&](uint8_t* set, const unsigned mask, const int k, double& sxx, double& sxy, double& syy) {
     sxx = sxy = syy = 0.0;
     if (!((mask >> k) & 1u)) return;
     const int slot = tid + k * T;
 #pragma unroll
-    for (int p = 0; p < kPatchArea; ++p) {
-      const float2 gr = pd[p * SA + slot];
-      const double dx = (double)gr.x, dy = (double)gr.y;
-      sxx = fma(dx, dx, sxx);
-      sxy = fma(dx, dy, sxy);
-      syy = fma(dy, dy, syy);
+    for (int j = 0; j < 8; ++j) {  // gradient chunk j: pixels 2j, 2j + 1
+      const float4 gr = *pchunk(set, slot, 4 + j);
+      const double dx0 = (double)gr.x, dy0 = (double)gr.y, dx1 = (double)gr.z, dy1 = (double)gr.w;
+      sxx = fma(dx0, dx0, sxx);
+      sxy = fma(dx0, dy0, sxy);
+      syy = fma(dy0, dy0, syy);
+      sxx = fma(dx1, dx1, sxx);
+      sxy = fma(dx1, dy1, sxy);
+      syy = fma(dy1, dy1, syy);
     }
   };
-  auto patch_moments = [&](const float2* pd, const unsigned mask, double (&sxx)[FPT], double (&sxy)[FPT], double (&syy)[FPT]) {
+  auto patch_moments = [&](uint8_t* set, const unsigned mask, double (&sxx)[FPT], double (&sxy)[FPT], double (&syy)[FPT]) {
 #pragma unroll
-    for (int k = 0; k < FPT; ++k) feat_moments(pd, mask, k, sxx[k], sxy[k], syy[k]);
+    for (int k = 0; k < FPT; ++k) feat_moments(set, mask, k, sxx[k], sxy[k], syy[k]);
   };
-  // ---- precomputeReferencePatches (:84-145) of one level into the patch arrays (pr, pd): visibility bits, the f32 patch and
+  // ---- precomputeReferencePatches (:84-145) of one level into the patch array set `set`: visibility bits, the f32 patch and
   //      its gradients, and the per-feature gradient moments m_* the H reduction needs.  `with_windows`: also request the
   //      current-image windows (between the footprint loads and the arithmetic, so that both latencies overlap).
   //      Throughput geometry: the loop over the thread's features is not unrolled, so moments stored here would be indexed by
   //      the feature and live in local memory, which misses the small L1 left beside 3 x 75 KB of shared memory; it leaves
-  //      m_* alone and the H sum takes them from pd with feat_moments(pd, vis_mask) -- a visible patch has its gradients
-  //      in pd (zero for a stale one), summed in the same order.  The other geometries unroll the loop and keep the moments of
-  //      the patch arithmetic (a second pass over pd would lengthen the latency path of the cluster geometries).
-  auto level_patches = [&](const int level, float* pr, float2* pd, const float* pr_stale, const int mode, const bool with_windows,
+  //      m_* alone and the H sum takes them from the set with feat_moments(set, vis_mask) -- a visible patch has its
+  //      gradients there (zero for a stale one), summed in the same order.  The other geometries unroll the loop and keep the moments of
+  //      the patch arithmetic (a second pass over the gradients would lengthen the latency path of the cluster geometries).
+  auto level_patches = [&](const int level, uint8_t* set, uint8_t* set_stale, const int mode, const bool with_windows,
                            double (&m_sxx)[FPT], double (&m_sxy)[FPT], double (&m_syy)[FPT]) {
     const int W = P.w[level], Hh = P.h[level];
     const float scale = 1.0f / (float)(1 << level);
@@ -1127,18 +1130,18 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
           for (int c = 0; c < 6; ++c) b2[c] = bilin(wtl, wtr, wbl, wbr, pr0[c], pr0[c + 1], pr1[c], pr1[c + 1]);
           if (r >= 2) {  // rows b0 (= Bq[y]), b1 (= Bq[y+1]), b2 (= Bq[y+2]) with y = r-2 are complete
             const int y = r - 2;
+            float dx[4], dy[4];
 #pragma unroll
             for (int x = 0; x < 4; ++x) {
-              const int p = y * 4 + x;
-              const float val = b1[x + 1];
-              const float dx = __fmul_rn(0.5f, __fsub_rn(b1[x + 2], b1[x]));
-              const float dy = __fmul_rn(0.5f, __fsub_rn(b2[x + 1], b0[x + 1]));
-              pr[p * SA + slot] = val;
-              pd[p * SA + slot] = make_float2(dx, dy);
-              sxx = fma((double)dx, (double)dx, sxx);
-              sxy = fma((double)dx, (double)dy, sxy);
-              syy = fma((double)dy, (double)dy, syy);
+              dx[x] = __fmul_rn(0.5f, __fsub_rn(b1[x + 2], b1[x]));
+              dy[x] = __fmul_rn(0.5f, __fsub_rn(b2[x + 1], b0[x + 1]));
+              sxx = fma((double)dx[x], (double)dx[x], sxx);
+              sxy = fma((double)dx[x], (double)dy[x], sxy);
+              syy = fma((double)dy[x], (double)dy[x], syy);
             }
+            *pchunk(set, slot, y) = make_float4(b1[1], b1[2], b1[3], b1[4]);
+            *pchunk(set, slot, 4 + 2 * y) = make_float4(dx[0], dy[0], dx[1], dy[1]);
+            *pchunk(set, slot, 5 + 2 * y) = make_float4(dx[2], dy[2], dx[3], dy[3]);
           }
 #pragma unroll
           for (int c = 0; c < 6; ++c) { b0[c] = b1[c]; b1[c] = b2[c]; }
@@ -1151,9 +1154,9 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         // and a zeroed Jacobian (jacobian_cache_.setZero() per level, :64).  Unreachable for
         // dyadic pyramids (SURVEY.md quirk 1) but kept bit-faithful.
 #pragma unroll
-        for (int p = 0; p < kPatchArea; ++p) pd[p * SA + slot] = make_float2(0.f, 0.f);
-        if (pr_stale)  // per-level arrays (upfront variant): the stale patch is the previous level's
-          for (int p = 0; p < kPatchArea; ++p) pr[p * SA + slot] = pr_stale[p * SA + slot];
+        for (int j = 0; j < 8; ++j) *pchunk(set, slot, 4 + j) = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (set_stale)  // per-level arrays (upfront variant): the stale patch is the previous level's
+          for (int y = 0; y < 4; ++y) *pchunk(set, slot, y) = *pchunk(set_stale, slot, y);
       }
     }
   };
@@ -1169,7 +1172,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     for (int level = lvl_hi; level >= lvl_lo; --level) {
       const int li = lvl_hi - level;
       double m_sxx[FPT], m_sxy[FPT], m_syy[FPT];
-      level_patches(level, pat_ref_of(li), pat_dxy_of(li), li > 0 ? pat_ref_of(li - 1) : (const float*)nullptr, kModeGlobal, false,
+      level_patches(level, pat_of(li), li > 0 ? pat_of(li - 1) : (uint8_t*)nullptr, kModeGlobal, false,
                     m_sxx, m_sxy, m_syy);
       vis_levels |= (vis_mask & 1u) << li;
       warp_h_partials<FPT, false>(
@@ -1240,7 +1243,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       // ---- precomputeReferencePatches (:84-145), one feature per thread; the windows of the current image are requested
       //      between the footprint loads and the patch arithmetic
       double m_sxx[FPT], m_sxy[FPT], m_syy[FPT];
-      level_patches(level, pat_ref, pat_dxy, (const float*)nullptr, mode, true, m_sxx, m_sxy, m_syy);
+      level_patches(level, pat, (uint8_t*)nullptr, mode, true, m_sxx, m_sxy, m_syy);
       SIA_DBG(if ((SVO_SIA_DEBUG && P.debug) && tid == 0) { tq1 = clock64(); s.tk[7] += tq1 - tq0; })
       // Only fwarp waits for the other warps' H partials (!EVAL: a named barrier the others arrive on and pass).  fwarp
       // reads s.hpart before it reaches barrier A of iteration 0, and nothing rewrites s.hpart -- the slow path's sum, the
@@ -1250,7 +1253,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       pair_sum_h_to_warp0<FPT, CS, XG, SS, SH, !EVAL>(
           [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
             { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); }
-            if constexpr (SS) feat_moments(pat_dxy, vis_mask, k, sxx, sxy, syy);
+            if constexpr (SS) feat_moments(pat, vis_mask, k, sxx, sxy, syy);
             else { sxx = sel_k(m_sxx, k); sxy = sel_k(m_sxy, k); syy = sel_k(m_syy, k); }
             cnt = ((vis_mask >> k) & 1u) ? 1.0 : 0.0;
             // opaque to the optimiser: otherwise the level-invariant Jacobian rows are hoisted out of the level loop and
@@ -1270,8 +1273,7 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
     } else {
       // everything pose independent was prepared before the first level: select this level's arrays, request the windows
       const int li = lvl_hi - level;
-      pat_ref = pat_ref_of(li);
-      pat_dxy = pat_dxy_of(li);
+      pat = pat_of(li);
       sol_level = &up.sol[li];
       vis_mask = (vis_levels >> li) & 1u;
 #pragma unroll
@@ -1359,16 +1361,18 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
         for (int yy = 0; yy < 4; ++yy) {
           q1[0] = byte_to_float<0>(lo[yy + 1]); q1[1] = byte_to_float<1>(lo[yy + 1]); q1[2] = byte_to_float<2>(lo[yy + 1]);
           q1[3] = byte_to_float<3>(lo[yy + 1]); q1[4] = byte_to_float<0>(hi[yy + 1]);
+          // patch row yy: its values and gradients, three 128-bit loads (one row at a time: at most 12 more live floats)
+          const float4 pv = *pchunk(pat, slot, yy), pg0 = *pchunk(pat, slot, 4 + 2 * yy), pg1 = *pchunk(pat, slot, 5 + 2 * yy);
+          const float val_r[4] = {pv.x, pv.y, pv.z, pv.w};
+          const float gx_r[4] = {pg0.x, pg0.z, pg1.x, pg1.z}, gy_r[4] = {pg0.y, pg0.w, pg1.y, pg1.w};
 #pragma unroll
           for (int xx = 0; xx < 4; ++xx) {
             const int p = yy * 4 + xx;
             const float I = bilin(wtl, wtr, wbl, wbr, q0[xx], q0[xx + 1], q1[xx], q1[xx + 1]);
-            const float val = pat_ref[p * SA + slot];
-            const float2 gr = pat_dxy[p * SA + slot];
-            const float res = __fsub_rn(I, val);
+            const float res = __fsub_rn(I, val_r[xx]);
             c2 = fmaf(res, res, c2);  // chi2 += res*res*weight, weight == 1 (:222); order differs from the serial sum anyway
-            gx = fmaf(gr.x, res, gx);
-            gy = fmaf(gr.y, res, gy);
+            gx = fmaf(gx_r[xx], res, gx);
+            gy = fmaf(gy_r[xx], res, gy);
             if (EVAL) P.residuals_out[(size_t)(fbase + slot) * kPatchArea + p] = res;
           }
 #pragma unroll
@@ -1445,13 +1449,13 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
       // contributed in this pass ("slow path"; all threads, one block barrier inside)
       auto slow_sum_h = [&]() {
         double q_sxx[FPT], q_sxy[FPT], q_syy[FPT];
-        if constexpr (!SS) patch_moments(pat_dxy, in_mask, q_sxx, q_sxy, q_syy);
+        if constexpr (!SS) patch_moments(pat, in_mask, q_sxx, q_sxy, q_syy);
         pair_sum_h_to_warp0<FPT, CS, XG, SS, SH>(
             [&](int k, double& x, double& y, double& zi, double& sxx, double& sxy, double& syy, double& cnt) {
               // a feature outside the image contributes nothing, also where its Jacobian rows are not finite (a point at
               // zero depth, or with f_z == 0): 1/z is selected away, the rows are then finite and the moments zero
               { double z_; feat_xyz(k, (int)threadIdx.x + k * (int)blockDim.x, x, y, z_); zi = feat_zi(k, z_); }
-              if constexpr (SS) feat_moments(pat_dxy, in_mask, k, sxx, sxy, syy);
+              if constexpr (SS) feat_moments(pat, in_mask, k, sxx, sxy, syy);
               else { sxx = sel_k(q_sxx, k); sxy = sel_k(q_sxy, k); syy = sel_k(q_syy, k); }
               cnt = 0.0;
               asm volatile("" : "+d"(x), "+d"(y), "+d"(zi));  // see the per-level call: no hoisting into local memory
@@ -1561,8 +1565,11 @@ __global__ void __launch_bounds__(MAXT, MINB) sia_kernel(const SiaParams P) {
             if (!((vis_mask >> k) & 1u))
               for (int p = 0; p < kPatchArea; ++p)
                 P.residuals_out[(size_t)(fbase + i) * kPatchArea + p] = __int_as_float(0x7fc00000);
-            for (int p = 0; p < kPatchArea; ++p)
-              P.ref_patch_out[(size_t)(fbase + i) * kPatchArea + p] = pat_ref[p * SA + i];
+            for (int y = 0; y < 4; ++y) {
+              const float4 v = *pchunk(pat, i, y);
+              float* o = P.ref_patch_out + (size_t)(fbase + i) * kPatchArea + 4 * y;
+              o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+            }
           }
         }
         break;
