@@ -209,6 +209,13 @@ struct PoObs {
   uint8_t* valid;
 };
 
+// rcp_rn seeds its Newton steps with the f32 reciprocal: inside (1e-30, 1e30) that seed is finite and nonzero and the
+// result is the correctly rounded 1/d; outside it (or for 0, inf, NaN) the seed is 0 or inf and only IEEE division is 1/d.
+__device__ __forceinline__ bool rcp_in_range(double d) {
+  const double a = fabs(d);
+  return a > 1e-30 && a < 1e30;
+}
+
 // e = (project2d(f) - project2d(T_f_w * pos)) / (1 << level)  (:52-54, :82-85, :135-137); xyz_f out
 __device__ __forceinline__ void reproj_error(const PoObs& o, int i, const double (&R)[9], const double (&t)[3], double& ex,
                                              double& ey, double (&p)[3], double& z_inv) {
@@ -216,10 +223,19 @@ __device__ __forceinline__ void reproj_error(const PoObs& o, int i, const double
   p[0] = R[0] * X + R[1] * Y + R[2] * Z + t[0];
   p[1] = R[3] * X + R[4] * Y + R[5] * Z + t[1];
   p[2] = R[6] * X + R[7] * Y + R[8] * Z + t[2];
-  z_inv = rcp_rn(p[2]);
   const double sic = o.sic[i];
-  ex = (o.fxn[i] - div_rn(p[0], p[2], z_inv)) * sic;
-  ey = (o.fyn[i] - div_rn(p[1], p[2], z_inv)) * sic;
+  double qx, qy;
+  if (rcp_in_range(p[2])) {
+    z_inv = rcp_rn(p[2]);
+    qx = div_rn(p[0], p[2], z_inv);
+    qy = div_rn(p[1], p[2], z_inv);
+  } else {  // a point on, behind-and-near or far beyond the camera plane: the reference's IEEE division
+    z_inv = 1.0 / p[2];
+    qx = p[0] / p[2];
+    qy = p[1] / p[2];
+  }
+  ex = (o.fxn[i] - qx) * sic;
+  ey = (o.fyn[i] - qy) * sic;
 }
 
 __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
@@ -315,7 +331,8 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
   // ---- Gauss-Newton (:63-121) -------------------------------------------------------------------
   for (int iter = 0; iter < P.n_iter; ++iter) {
     if (iter == 5) scale = 0.85 / fx;  // (:69-70)
-    const double scale_rcp = rcp_rn(scale);
+    const bool scale_fast = rcp_in_range(scale);  // a float-subnormal or zero MAD scale divides by IEEE rules
+    const double scale_rcp = scale_fast ? rcp_rn(scale) : 0.0;
     double acc[kPoK];
 #pragma unroll
     for (int k = 0; k < kPoK; ++k) acc[k] = 0.0;
@@ -333,7 +350,8 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(PoseOptParams P) {
       for (int k = 0; k < 6; ++k) { J0[k] *= sic; J1[k] *= sic; }
       const double e_sq = ex * ex + ey * ey;
       if (iter == 0) o.init[i] = e_sq;  // chi2_vec_init (:87-88)
-      const double w = (double)tukey_weight((float)div_rn(sqrt(e_sq), scale, scale_rcp));  // e.norm() / scale, correctly rounded
+      const double en = sqrt(e_sq);
+      const double w = (double)tukey_weight((float)(scale_fast ? div_rn(en, scale, scale_rcp) : en / scale));  // e.norm() / scale, correctly rounded
       int idx = 0;
 #pragma unroll
       for (int r = 0; r < 6; ++r)
@@ -512,7 +530,7 @@ extern "C" int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double rep
   if (!ctx || B < 0 || n_iter < 0 || (B > 0 && (!fx || !T_f_w_io || !obs_offset || !out)))
     return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: bad arguments");
   if (B == 0) return 0;
-  memset(out, 0, sizeof(*out) * (size_t)B);
+  // every check comes before anything is written: a refused call leaves out, T_f_w_io and has_point_io as they were
   const int base = obs_offset[0], total = obs_offset[B] - base;
   if (base < 0) return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: obs_offset[0] is negative");
   int max_n = 0;
@@ -521,12 +539,18 @@ extern "C" int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double rep
     if (n < 0) return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: obs_offset not monotone");
     if (n > max_n) max_n = n;
   }
-  if (total == 0) return 0;  // errors.empty() -> return, for every frame
-  if (!f || !point_pos || !level || !has_point_io) return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: NULL observation arrays");
-  cudaSetDevice(ctx->device);
+  if (total > 0 && (!f || !point_pos || !level || !has_point_io))
+    return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: NULL observation arrays");
+  // sqrt_inv_cov = 1.0 / (1 << level) is defined for levels 0..30 only
+  for (int i = base; i < base + total; ++i)
+    if (has_point_io[i] && (level[i] < 0 || level[i] > 30))
+      return set_err(ctx, SVO_B200_EINVAL, "pose_optimize_batch: observation %d has level %d outside [0, 30]", i - base, level[i]);
   const size_t smem = ((sizeof(PoseOptShared) + 15) & ~size_t(15)) + (sizeof(double) * 8 + 1) * (size_t)((max_n + 1) & ~1) + 16;
   if (smem > (size_t)ctx->max_smem_optin)
     return set_err(ctx, SVO_B200_ELIMIT, "pose_optimize: %d observations in one frame need %zu B of shared memory", max_n, smem);
+  memset(out, 0, sizeof(*out) * (size_t)B);
+  if (total == 0) return 0;  // errors.empty() -> return, for every frame
+  cudaSetDevice(ctx->device);
   Carver c;
   const size_t o_T = c.take(sizeof(double) * 12 * B), o_hp = c.take(total), o_out = c.take(sizeof(svo_b200_pose_opt_result) * B);
   const size_t io_end = c.off;
