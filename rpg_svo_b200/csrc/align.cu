@@ -9,6 +9,7 @@
 // and one launch aligns them all.  Per-feature state (10x10 template, gradients, residuals) lives in a
 // per-warp slice of shared memory; see warp_align.cuh for the arithmetic contract.
 #include <cstring>
+#include <vector>
 
 #include "ctx.h"
 #include "warp_align.cuh"
@@ -103,38 +104,28 @@ static int align_batch(svo_b200_ctx* ctx, const svo_b200_frame* cur, int M, cons
     if (level[m] < 0 || level[m] >= cur->n_levels)
       return set_err(ctx, SVO_B200_EINVAL, "align_batch: level[%d]=%d outside the pyramid", m, level[m]);
   cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_lvl = c.take(sizeof(int) * M), o_dir = c.take(dir ? sizeof(float) * 2 * M : 0),
-               o_pwb = c.take((size_t)100 * M), o_pat = c.take((size_t)64 * M), o_px = c.take(sizeof(double) * 2 * M);
-  const size_t in_bytes = c.off;
-  const size_t o_conv = c.take(M), o_h = c.take(sizeof(double) * M);
+  Staging st(ctx);
+  const int* d_level;
+  const float* d_dir = nullptr;  // 2D: no direction
+  const uint8_t *d_pwb, *d_patch;
+  double *d_px, *d_h_inv = nullptr;
+  uint8_t* d_conv;
+  st.in(level, M, &d_level);
+  if (dir) st.in(dir, 2 * (size_t)M, &d_dir);
+  st.in(pwb, 100 * (size_t)M, &d_pwb);
+  st.in(patch, 64 * (size_t)M, &d_patch);
+  st.inout(px_io, 2 * (size_t)M, &d_px);
+  st.out(converged_out, M, &d_conv);
+  if (h_inv_out) st.out(h_inv_out, M, &d_h_inv);
   int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_lvl, level, sizeof(int) * M);
-  if (dir) memcpy(h + o_dir, dir, sizeof(float) * 2 * M);
-  memcpy(h + o_pwb, pwb, (size_t)100 * M);
-  memcpy(h + o_pat, patch, (size_t)64 * M);
-  memcpy(h + o_px, px_io, sizeof(double) * 2 * M);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = st.open()) || (rc = st.send())) return rc;
   const int blocks = (M + kWarpsPerCta - 1) / kWarpsPerCta;
-  kt_begin(ctx);
-  align_batch_kernel<<<blocks, kWarpsPerCta * 32, 0, ctx->stream>>>(
-      make_desc(cur), M, reinterpret_cast<const int*>(d + o_lvl), dir ? reinterpret_cast<const float*>(d + o_dir) : nullptr,
-      d + o_pwb, d + o_pat, n_iter, reinterpret_cast<double*>(d + o_px), d + o_conv,
-      h_inv_out ? reinterpret_cast<double*>(d + o_h) : nullptr);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_px, d + o_px, c.off - o_px, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(px_io, h + o_px, sizeof(double) * 2 * M);
-  memcpy(converged_out, h + o_conv, M);
-  if (h_inv_out) memcpy(h_inv_out, h + o_h, sizeof(double) * M);
-  return 0;
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         align_batch_kernel<<<blocks, kWarpsPerCta * 32, 0, ctx->stream>>>(make_desc(cur), M, d_level, d_dir, d_pwb, d_patch, n_iter,
+                                                                           d_px, d_conv, d_h_inv);
+       })))
+    return rc;
+  return st.receive();
 }
 
 }  // namespace svo
@@ -172,69 +163,41 @@ int svo_b200_find_match_direct(svo_b200_ctx* ctx, const svo_b200_frame* const* r
     if (!ref_frames[r]) return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: ref_frames[%d] is NULL", r);
   if (!ref_index || !ref_px || !ref_f || !ref_level || !ftr_type || !ref_grad || !point_pos || !px_cur_io || !success_out)
     return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: NULL candidate arrays");
-  for (int m = 0; m < M; ++m) {
-    if (ref_index[m] < 0 || ref_index[m] >= n_ref)
-      return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: ref_index[%d] out of range", m);
-    if (ref_level[m] < 0 || ref_level[m] >= ref_frames[ref_index[m]]->n_levels)
-      return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: ref_level[%d] outside the pyramid", m);
-  }
-  if (opt->max_search_level >= cur->n_levels)
-    return set_err(ctx, SVO_B200_EINVAL, "find_match_direct: max_search_level %d >= %d pyramid levels",
-                   opt->max_search_level, cur->n_levels);
-  if (const int rc_sz = cam_check_frames(ctx, "find_match_direct", cam, &cur, 1)) return rc_sz;
-  if (const int rc_sz = cam_check_frames(ctx, "find_match_direct", cam, ref_frames, n_ref)) return rc_sz;
-  cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),
-               o_lv = c.take(sizeof(int) * M), o_ty = c.take(sizeof(int) * M), o_gr = c.take(sizeof(double) * 2 * M),
-               o_pp = c.take(sizeof(double) * 3 * M), o_rT = c.take(sizeof(double) * 12 * n_ref),
-               o_cT = c.take(sizeof(double) * 12), o_fr = c.take(sizeof(FrameDesc) * n_ref),
-               o_pc = c.take(sizeof(double) * 2 * M);
-  const size_t in_bytes = c.off;
-  const size_t o_su = c.take(M), o_sl = c.take(sizeof(int) * M), o_A = c.take(sizeof(double) * 4 * M),
-               o_h = c.take(sizeof(double) * M);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_ri, ref_index, sizeof(int) * M);
-  memcpy(h + o_px, ref_px, sizeof(double) * 2 * M);
-  memcpy(h + o_f, ref_f, sizeof(double) * 3 * M);
-  memcpy(h + o_lv, ref_level, sizeof(int) * M);
-  memcpy(h + o_ty, ftr_type, sizeof(int) * M);
-  memcpy(h + o_gr, ref_grad, sizeof(double) * 2 * M);
-  memcpy(h + o_pp, point_pos, sizeof(double) * 3 * M);
-  memcpy(h + o_rT, ref_T_f_w, sizeof(double) * 12 * n_ref);
-  memcpy(h + o_cT, cur_T_f_w, sizeof(double) * 12);
-  for (int r = 0; r < n_ref; ++r) reinterpret_cast<FrameDesc*>(h + o_fr)[r] = make_desc(ref_frames[r]);
-  memcpy(h + o_pc, px_cur_io, sizeof(double) * 2 * M);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  MatchIn in = {reinterpret_cast<const int*>(d + o_ri), reinterpret_cast<const double*>(d + o_px),
-                reinterpret_cast<const double*>(d + o_f), reinterpret_cast<const int*>(d + o_lv),
-                reinterpret_cast<const int*>(d + o_ty), reinterpret_cast<const double*>(d + o_gr),
-                reinterpret_cast<const double*>(d + o_pp), reinterpret_cast<const double*>(d + o_rT),
-                reinterpret_cast<const FrameDesc*>(d + o_fr)};
-  MatchOut out = {reinterpret_cast<double*>(d + o_pc), d + o_su, reinterpret_cast<int*>(d + o_sl),
-                  reinterpret_cast<double*>(d + o_A), reinterpret_cast<double*>(d + o_h)};
+  int rc = check_ref_table(ctx, "find_match_direct", "ref_level", ref_frames, n_ref, M, ref_index, ref_level, cur, cam,
+                           opt->max_search_level);
+  if (rc) return rc;
   Cam cm;
-  { const int rc_cam = cam_to_dev(ctx, cam, cm); if (rc_cam) return rc_cam; }
+  if ((rc = cam_to_dev(ctx, cam, cm))) return rc;
+  cudaSetDevice(ctx->device);
+  std::vector<FrameDesc> frames((size_t)n_ref);
+  for (int r = 0; r < n_ref; ++r) frames[r] = make_desc(ref_frames[r]);
+  Staging st(ctx);
+  MatchIn in;
+  MatchOut out;
+  const double* d_cur_T;
+  st.in(ref_index, M, &in.ref_index);
+  st.in(ref_px, 2 * (size_t)M, &in.ref_px);
+  st.in(ref_f, 3 * (size_t)M, &in.ref_f);
+  st.in(ref_level, M, &in.ref_level);
+  st.in(ftr_type, M, &in.ftr_type);
+  st.in(ref_grad, 2 * (size_t)M, &in.ref_grad);
+  st.in(point_pos, 3 * (size_t)M, &in.point_pos);
+  st.in(ref_T_f_w, 12 * (size_t)n_ref, &in.ref_T_f_w);
+  st.in(cur_T_f_w, 12, &d_cur_T);
+  st.in(frames.data(), n_ref, &in.ref_frames);
+  st.inout(px_cur_io, 2 * (size_t)M, &out.px_cur);
+  st.out(success_out, M, &out.success);
+  st.out(search_level_out, M, &out.search_level);
+  st.out(A_cur_ref_out, 4 * (size_t)M, &out.A_cur_ref);
+  st.out(h_inv_out, M, &out.h_inv);
+  if ((rc = st.open()) || (rc = st.send())) return rc;
   const int blocks = (M + kWarpsPerCta - 1) / kWarpsPerCta;
-  kt_begin(ctx);
-  find_match_direct_kernel<<<blocks, kWarpsPerCta * 32, 0, ctx->stream>>>(
-      make_desc(cur), cm, M, in, out, opt->max_search_level, opt->align_max_iter, reinterpret_cast<const double*>(d + o_cT));
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_pc, d + o_pc, c.off - o_pc, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(px_cur_io, h + o_pc, sizeof(double) * 2 * M);
-  memcpy(success_out, h + o_su, M);
-  if (search_level_out) memcpy(search_level_out, h + o_sl, sizeof(int) * M);
-  if (A_cur_ref_out) memcpy(A_cur_ref_out, h + o_A, sizeof(double) * 4 * M);
-  if (h_inv_out) memcpy(h_inv_out, h + o_h, sizeof(double) * M);
-  return 0;
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         find_match_direct_kernel<<<blocks, kWarpsPerCta * 32, 0, ctx->stream>>>(make_desc(cur), cm, M, in, out, opt->max_search_level,
+                                                                                 opt->align_max_iter, d_cur_T);
+       })))
+    return rc;
+  return st.receive();
 }
 
 }  // extern "C"

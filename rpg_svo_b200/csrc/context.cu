@@ -90,6 +90,70 @@ int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes) {
   return 0;
 }
 
+int Staging::open() {
+  Carver c;
+  const auto lay = [&](bool in, bool back) {
+    for (Region& r : regions_)
+      if (r.in == in && r.back == back) r.off = c.take(r.bytes, r.align);
+  };
+  lay(true, false);
+  front_ = c.off;
+  back_ = c.take(0);
+  lay(true, true);
+  if (c.off > back_) front_ = c.off;
+  lay(false, true);
+  end_ = c.off;
+  int rc;
+  if ((rc = ensure_host(ctx_, ctx_->h_in, end_))) return rc;
+  if ((rc = ensure_dev(ctx_, ctx_->d_in, end_))) return rc;
+  SVO_CUDA_CHECK(ctx_, cudaStreamSynchronize(ctx_->stream));
+  h_ = static_cast<uint8_t*>(ctx_->h_in.p);
+  d_ = static_cast<uint8_t*>(ctx_->d_in.p);
+  for (const Region& r : regions_) r.bind(r.at, d_ + r.off);
+  for (const Region& r : regions_)
+    if (r.in && r.src && r.bytes) memcpy(h_ + r.off, r.src, r.bytes);
+  return 0;
+}
+
+int Staging::send() {
+  SVO_CUDA_CHECK(ctx_, cudaMemcpyAsync(d_, h_, front_, cudaMemcpyHostToDevice, ctx_->stream));
+  return 0;
+}
+
+int Staging::receive() {
+  SVO_CUDA_CHECK(ctx_, cudaMemcpyAsync(h_ + back_, d_ + back_, end_ - back_, cudaMemcpyDeviceToHost, ctx_->stream));
+  SVO_CUDA_CHECK(ctx_, cudaStreamSynchronize(ctx_->stream));
+  for (const Region& r : regions_)
+    if (r.back && r.dst && r.bytes) memcpy(r.dst, h_ + r.off, r.bytes);
+  return 0;
+}
+
+int entry_err(svo_b200_ctx* ctx, int rc, const char* name, const char* what, int i) {
+  if (!ctx || !name) return rc;
+  const std::string why = ctx->err;
+  return set_err(ctx, rc, "%s: %s %d: %s", name, what, i, why.c_str());
+}
+
+int check_ref_levels(svo_b200_ctx* ctx, const char* who, const char* level_name, const svo_b200_frame* const* ref_frames,
+                     int n_ref, int M, const int* ref_index, const int* level) {
+  for (int m = 0; m < M; ++m) {
+    if (ref_index[m] < 0 || ref_index[m] >= n_ref) return set_err(ctx, SVO_B200_EINVAL, "%s: ref_index[%d] out of range", who, m);
+    if (level[m] < 0 || level[m] >= ref_frames[ref_index[m]]->n_levels)
+      return set_err(ctx, SVO_B200_EINVAL, "%s: %s[%d] outside the pyramid", who, level_name, m);
+  }
+  return 0;
+}
+
+int check_ref_table(svo_b200_ctx* ctx, const char* who, const char* level_name, const svo_b200_frame* const* ref_frames,
+                    int n_ref, int M, const int* ref_index, const int* level, const svo_b200_frame* cur,
+                    const svo_b200_camera* cam, int max_search_level) {
+  if (const int rc = check_ref_levels(ctx, who, level_name, ref_frames, n_ref, M, ref_index, level)) return rc;
+  if (max_search_level >= cur->n_levels)
+    return set_err(ctx, SVO_B200_EINVAL, "%s: max_search_level %d >= %d pyramid levels", who, max_search_level, cur->n_levels);
+  if (const int rc = cam_check_frames(ctx, who, cam, &cur, 1)) return rc;
+  return cam_check_frames(ctx, who, cam, ref_frames, n_ref);
+}
+
 // [EXT] vk::halfSample (svo/src/frame.cpp:156-165), both branches of rpg_vikit's vision.cpp:
 //   scalar: out = (a + b + c + d) / 4, integer division;
 //   SSE2 (what an x86 build runs when in_w % 16 == 0): vertical _mm_avg_epu8, then _mm_avg_epu16 of adjacent columns,
@@ -650,10 +714,8 @@ void svo_b200_destroy(svo_b200_ctx* ctx) {
   sia_batch_free(ctx);
   sia_split_free(ctx);
   if (ctx->d_in.p) cudaFree(ctx->d_in.p);
-  if (ctx->d_out.p) cudaFree(ctx->d_out.p);
   if (ctx->d_scratch.p) cudaFree(ctx->d_scratch.p);
   if (ctx->h_in.p) cudaFreeHost(ctx->h_in.p);
-  if (ctx->h_out.p) cudaFreeHost(ctx->h_out.p);
   if (ctx->ev_k0) cudaEventDestroy(ctx->ev_k0);
   if (ctx->ev_k1) cudaEventDestroy(ctx->ev_k1);
   cudaStreamDestroy(ctx->stream);

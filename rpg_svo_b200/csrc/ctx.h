@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/svo_b200.h"
@@ -68,9 +69,9 @@ struct svo_b200_ctx {
   uint64_t launches = 0;
   int sm_count = 0;
   int max_smem_optin = 0;
-  // generic scratch (each entry point carves what it needs)
-  DevBuf d_in, d_out, d_scratch;
-  HostBuf h_in, h_out;
+  // generic scratch: h_in / d_in hold an entry point's Staging, d_scratch the device-only arrays some carve
+  DevBuf d_in, d_scratch;
+  HostBuf h_in;
   svo::SiaBatchState* sia = nullptr;
   cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around the kernel(s) of the last entry point (svo_b200_last_kernel_ms)
   int pyramid_rule = SVO_B200_PYR_X86;  // svo_b200_set_pyramid_rule
@@ -139,6 +140,85 @@ inline void kt_begin(svo_b200_ctx* ctx) {
   if (ctx->ev_k0) cudaEventRecord(ctx->ev_k0, ctx->stream);
 }
 inline void kt_end(svo_b200_ctx* ctx) { if (ctx->ev_k1) cudaEventRecord(ctx->ev_k1, ctx->stream); }
+
+// The kernel launches of an entry point: `launch` enqueues n of them between kt_begin and kt_end; they are counted for
+// svo_b200_launch_count and their launch error is returned.
+template <class F>
+int launch_kernels(svo_b200_ctx* ctx, int n, F&& launch) {
+  kt_begin(ctx);
+  launch();
+  ctx->launches += n;
+  kt_end(ctx);
+  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  return 0;
+}
+
+// An entry point's arrays staged through the context's pinned buffer and its device mirror (h_in / d_in).  Each region is
+// declared once, by kind, element count and the pointer `at` that open() sets to its device address:
+//   in     copied in from src; a NULL src is filled by the caller through host() between open() and send();
+//   inout  copied in from io and back to it; a NULL io is filled and read by the caller;
+//   out    copied back to dst; a NULL dst is read by the caller through host(), or by nobody.
+// open() lays out the copied-in regions as one front range and the copied-back ones as one tail range (in-only, then
+// in-out, then out-only regions), grows the buffers, waits for the stream (an earlier copy may still read the pinned
+// buffer), sets every `at` and then copies the sources in, so that a table whose entries hold region addresses can itself
+// be a source.  send() copies the front range to the device; receive() copies the tail range back, waits for it and
+// copies every region with a destination out.
+class Staging {
+  template <class T>
+  struct same { using type = T; };
+  template <class T>
+  using same_t = typename same<T>::type;  // element types come from `at` alone
+
+ public:
+  explicit Staging(svo_b200_ctx* ctx) : ctx_(ctx) {}
+  template <class T>
+  void in(const same_t<T>* src, size_t n, T** at, size_t align = 256) { add(src, nullptr, sizeof(T) * n, align, true, false, at); }
+  template <class T>
+  void inout(same_t<T>* io, size_t n, T** at, size_t align = 256) { add(io, io, sizeof(T) * n, align, true, true, at); }
+  template <class T>
+  void out(same_t<T>* dst, size_t n, T** at) { add(nullptr, dst, sizeof(T) * n, 256, false, true, at); }
+  int open();
+  int send();
+  int receive();
+  template <class T>
+  typename std::remove_const<T>::type* host(T* dev) const {  // the pinned mirror of a region's device address
+    return reinterpret_cast<typename std::remove_const<T>::type*>(h_ + (reinterpret_cast<const uint8_t*>(dev) - d_));
+  }
+  uint8_t* tail() const { return d_ + back_; }  // the device tail range, tail_bytes() long
+  size_t tail_bytes() const { return end_ - back_; }
+
+ private:
+  struct Region {
+    const void* src;
+    void* dst;
+    size_t bytes, align, off;
+    bool in, back;
+    void* at;
+    void (*bind)(void* at, uint8_t* p);
+  };
+  template <class T>
+  void add(const void* src, void* dst, size_t bytes, size_t align, bool in, bool back, T** at) {
+    regions_.push_back({src, dst, bytes, align, 0, in, back, at, [](void* a, uint8_t* p) { *static_cast<T**>(a) = reinterpret_cast<T*>(p); }});
+  }
+  svo_b200_ctx* ctx_;
+  std::vector<Region> regions_;
+  uint8_t *h_ = nullptr, *d_ = nullptr;
+  size_t front_ = 0, back_ = 0, end_ = 0;
+};
+
+// Re-prefixes the error that the check of entry i of a many-entry call left: "<name>: <what> <i>: <message>".  A single
+// call (name NULL) keeps the message.
+int entry_err(svo_b200_ctx* ctx, int rc, const char* name, const char* what, int i);
+
+// The candidates' reference features of the matcher entry points (`who`): every ref_index inside the n_ref keyframes and
+// every level (the array `level_name`) inside its keyframe's pyramid.
+int check_ref_levels(svo_b200_ctx* ctx, const char* who, const char* level_name, const svo_b200_frame* const* ref_frames,
+                     int n_ref, int M, const int* ref_index, const int* level);
+// check_ref_levels, then max_search_level below the current frame's levels and the camera's size that of cur and of
+// every keyframe.
+int check_ref_table(svo_b200_ctx* ctx, const char* who, const char* level_name, const svo_b200_frame* const* ref_frames,
+                    int n_ref, int M, const int* ref_index, const int* level, const svo_b200_frame* cur,
+                    const svo_b200_camera* cam, int max_search_level);
 
 // Device-side camera ([EXT] vk::PinholeCamera / vk::ATANCamera): the C-ABI parameters plus the derived constants
 // the vikit constructors precompute.  Passed by value inside kernel parameter structs.

@@ -391,134 +391,79 @@ int depth_run(svo_b200_ctx* ctx, const DepthParams& H, const svo_b200_frame* con
   const bool mo = H.match_only != 0;
   const bool general = !epi_is_default(ctx->epi);
   cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_ri = c.take(sizeof(int) * M), o_px = c.take(sizeof(double) * 2 * M), o_f = c.take(sizeof(double) * 3 * M),
-               o_lv = c.take(sizeof(int) * M), o_ty = c.take(sizeof(int) * M), o_gr = c.take(sizeof(double) * 2 * M),
-               o_rT = c.take(sizeof(double) * 12 * n_ref), o_fr = c.take(sizeof(FrameDesc) * n_ref),
-               o_tab = c.take(sizeof(DepthStream) * S), o_so = c.take(sizeof(int) * (S + 1));
-  size_t o_de = 0, o_dn = 0, o_dx = 0, o_bi = 0, o_zr = 0, o_a = 0, o_b = 0, o_mu = 0, o_s2 = 0;
-  if (mo) {  // the candidates' depth ranges
-    o_de = c.take(sizeof(double) * M); o_dn = c.take(sizeof(double) * M); o_dx = c.take(sizeof(double) * M);
-  } else {   // batch ids and z_range, then the seeds (copied both ways)
-    o_bi = c.take(sizeof(int) * M); o_zr = c.take(sizeof(float) * M);
-    o_a = c.take(sizeof(float) * M); o_b = c.take(sizeof(float) * M); o_mu = c.take(sizeof(float) * M);
-    o_s2 = c.take(sizeof(float) * M);
-  }
-  const size_t in_bytes = c.off;
-  const size_t o_st = c.take(M), o_pc = c.take(sizeof(double) * 2 * M), o_z = c.take(sizeof(double) * M),
-               o_nz = c.take(sizeof(int) * M);
-  size_t o_sl = 0, o_el = 0, o_rj = 0, o_A = 0, o_hi = 0, o_r1 = 0;
-  if (mo) {  // the Matcher's scratch members
-    o_sl = c.take(sizeof(int) * M); o_el = c.take(sizeof(double) * M); o_rj = c.take(M); o_A = c.take(sizeof(double) * 4 * M);
-    if (general) { o_hi = c.take(sizeof(double) * M); o_r1 = c.take(M); }  // h_inv_ (align1D runs only here)
-  }
-  const size_t o_back = mo ? o_st : o_a;
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_ri, H.ref_index, sizeof(int) * M);
-  memcpy(h + o_px, H.ftr_px, sizeof(double) * 2 * M);
-  memcpy(h + o_f, H.ftr_f, sizeof(double) * 3 * M);
-  memcpy(h + o_lv, H.ftr_level, sizeof(int) * M);
-  memcpy(h + o_ty, H.ftr_type, sizeof(int) * M);
-  memcpy(h + o_gr, H.ftr_grad, sizeof(double) * 2 * M);
-  memcpy(h + o_rT, ref_T_f_w, sizeof(double) * 12 * n_ref);
-  for (int r = 0; r < n_ref; ++r) reinterpret_cast<FrameDesc*>(h + o_fr)[r] = make_desc(ref_frames[r]);
-  memcpy(h + o_tab, streams, sizeof(DepthStream) * S);
-  memcpy(h + o_so, seed_offset, sizeof(int) * (S + 1));
-  if (mo) {
-    memcpy(h + o_de, H.d_est, sizeof(double) * M);
-    memcpy(h + o_dn, H.d_min, sizeof(double) * M);
-    memcpy(h + o_dx, H.d_max, sizeof(double) * M);
-  } else {
-    memcpy(h + o_bi, H.batch_id, sizeof(int) * M);
-    memcpy(h + o_zr, H.z_range, sizeof(float) * M);
-    memcpy(h + o_a, H.a, sizeof(float) * M);
-    memcpy(h + o_b, H.b, sizeof(float) * M);
-    memcpy(h + o_mu, H.mu, sizeof(float) * M);
-    memcpy(h + o_s2, H.sigma2, sizeof(float) * M);
-  }
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  if (mo) SVO_CUDA_CHECK(ctx, cudaMemsetAsync(d + o_st, 0, c.off - o_st, ctx->stream));
+  std::vector<FrameDesc> frames((size_t)n_ref);
+  for (int r = 0; r < n_ref; ++r) frames[r] = make_desc(ref_frames[r]);
+  Staging st(ctx);
   DepthParams P;
   memset(&P, 0, sizeof(P));
-  P.ref_frames = reinterpret_cast<const FrameDesc*>(d + o_fr);
-  P.ref_T_f_w = reinterpret_cast<const double*>(d + o_rT);
+  const DepthStream* d_streams;
+  const int* d_seed_offset;
+  st.in(H.ref_index, M, &P.ref_index);
+  st.in(H.ftr_px, 2 * (size_t)M, &P.ftr_px);
+  st.in(H.ftr_f, 3 * (size_t)M, &P.ftr_f);
+  st.in(H.ftr_level, M, &P.ftr_level);
+  st.in(H.ftr_type, M, &P.ftr_type);
+  st.in(H.ftr_grad, 2 * (size_t)M, &P.ftr_grad);
+  st.in(ref_T_f_w, 12 * (size_t)n_ref, &P.ref_T_f_w);
+  st.in(frames.data(), n_ref, &P.ref_frames);
+  st.in(streams, S, &d_streams);
+  st.in(seed_offset, S + 1, &d_seed_offset);
+  if (mo) {  // the candidates' depth ranges in; the status flags are converted on the way out
+    st.in(H.d_est, M, &P.d_est);
+    st.in(H.d_min, M, &P.d_min);
+    st.in(H.d_max, M, &P.d_max);
+    st.out<uint8_t>(nullptr, M, &P.status);
+  } else {   // batch ids and z_range in, the seeds both ways
+    st.in(H.batch_id, M, &P.batch_id);
+    st.in(H.z_range, M, &P.z_range);
+    st.inout(H.a, M, &P.a);
+    st.inout(H.b, M, &P.b);
+    st.inout(H.mu, M, &P.mu);
+    st.inout(H.sigma2, M, &P.sigma2);
+    st.out(H.status, M, &P.status);
+  }
+  st.out(H.px_cur, 2 * (size_t)M, &P.px_cur);
+  st.out(H.z, M, &P.z);
+  st.out(H.n_zmssd, M, &P.n_zmssd);
+  if (mo) {  // the Matcher's scratch members
+    st.out(H.search_level_out, M, &P.search_level_out);
+    st.out(H.epi_length_out, M, &P.epi_length_out);
+    st.out(H.reject_out, M, &P.reject_out);
+    st.out(H.A_out, 4 * (size_t)M, &P.A_out);
+    if (general) {  // h_inv_ (align1D runs only here)
+      st.out<double>(nullptr, M, &P.h_inv_out);
+      st.out<uint8_t>(nullptr, M, &P.ran_1d_out);
+    }
+  }
+  int rc;
+  if ((rc = st.open()) || (rc = st.send())) return rc;
+  if (mo) SVO_CUDA_CHECK(ctx, cudaMemsetAsync(st.tail(), 0, st.tail_bytes(), ctx->stream));
   P.M = M;
-  P.ref_index = reinterpret_cast<const int*>(d + o_ri);
-  P.ftr_px = reinterpret_cast<const double*>(d + o_px);
-  P.ftr_f = reinterpret_cast<const double*>(d + o_f);
-  P.ftr_level = reinterpret_cast<const int*>(d + o_lv);
-  P.ftr_type = reinterpret_cast<const int*>(d + o_ty);
-  P.ftr_grad = reinterpret_cast<const double*>(d + o_gr);
   P.max_n_kfs = opt->max_n_kfs;
   P.sigma2_thresh = opt->seed_convergence_sigma2_thresh;
   P.max_search_level = opt->max_search_level;
   P.align_max_iter = opt->align_max_iter;
   P.max_epi_search_steps = opt->max_epi_search_steps;
-  P.status = d + o_st;
-  P.px_cur = reinterpret_cast<double*>(d + o_pc);
-  P.z = reinterpret_cast<double*>(d + o_z);
-  P.n_zmssd = reinterpret_cast<int*>(d + o_nz);
   P.match_only = H.match_only;
-  if (mo) {
-    P.d_est = reinterpret_cast<const double*>(d + o_de);
-    P.d_min = reinterpret_cast<const double*>(d + o_dn);
-    P.d_max = reinterpret_cast<const double*>(d + o_dx);
-    P.search_level_out = reinterpret_cast<int*>(d + o_sl);
-    P.epi_length_out = reinterpret_cast<double*>(d + o_el);
-    P.reject_out = d + o_rj;
-    P.A_out = reinterpret_cast<double*>(d + o_A);
-    if (general) { P.h_inv_out = reinterpret_cast<double*>(d + o_hi); P.ran_1d_out = d + o_r1; }
-  } else {
-    P.batch_id = reinterpret_cast<const int*>(d + o_bi);
-    P.z_range = reinterpret_cast<float*>(d + o_zr);
-    P.a = reinterpret_cast<float*>(d + o_a);
-    P.b = reinterpret_cast<float*>(d + o_b);
-    P.mu = reinterpret_cast<float*>(d + o_mu);
-    P.sigma2 = reinterpret_cast<float*>(d + o_s2);
-  }
+  if (general) P.epi = ctx->epi;
   const int blocks = (M + kDfWarps - 1) / kDfWarps;
-  const DepthStream* d_streams = reinterpret_cast<const DepthStream*>(d + o_tab);
-  const int* d_seed_offset = reinterpret_cast<const int*>(d + o_so);
-  kt_begin(ctx);
-  if (general) {
-    P.epi = ctx->epi;
-    depth_filter_kernel<true><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
-  } else {
-    depth_filter_kernel<false><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
-  }
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_back, d + o_back, c.off - o_back, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         if (general) depth_filter_kernel<true><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
+         else depth_filter_kernel<false><<<blocks, kDfWarps * 32, 0, ctx->stream>>>(P, d_streams, d_seed_offset, S);
+       })))
+    return rc;
+  if ((rc = st.receive())) return rc;
   if (mo) {
-    for (int m = 0; m < M; ++m) H.status[m] = h[o_st + m] == SVO_B200_SEED_UPDATED;
-    if (H.search_level_out) memcpy(H.search_level_out, h + o_sl, sizeof(int) * M);
-    if (H.epi_length_out) memcpy(H.epi_length_out, h + o_el, sizeof(double) * M);
-    if (H.reject_out) memcpy(H.reject_out, h + o_rj, M);
-    if (H.A_out) memcpy(H.A_out, h + o_A, sizeof(double) * 4 * M);
+    const uint8_t* status = st.host(P.status);
+    for (int m = 0; m < M; ++m) H.status[m] = status[m] == SVO_B200_SEED_UPDATED;
     ctx->epi_h_inv.assign((size_t)M, 0.0);
     ctx->epi_ran_1d.assign((size_t)M, 0);
     if (general) {
-      memcpy(ctx->epi_h_inv.data(), h + o_hi, sizeof(double) * M);
-      memcpy(ctx->epi_ran_1d.data(), h + o_r1, M);
+      memcpy(ctx->epi_h_inv.data(), st.host(P.h_inv_out), sizeof(double) * M);
+      memcpy(ctx->epi_ran_1d.data(), st.host(P.ran_1d_out), M);
     }
     ctx->epi_last_valid = true;
-  } else {
-    memcpy(H.a, h + o_a, sizeof(float) * M);
-    memcpy(H.b, h + o_b, sizeof(float) * M);
-    memcpy(H.mu, h + o_mu, sizeof(float) * M);
-    memcpy(H.sigma2, h + o_s2, sizeof(float) * M);
-    memcpy(H.status, h + o_st, M);
   }
-  if (H.px_cur) memcpy(H.px_cur, h + o_pc, sizeof(double) * 2 * M);
-  if (H.z) memcpy(H.z, h + o_z, sizeof(double) * M);
-  if (H.n_zmssd) memcpy(H.n_zmssd, h + o_nz, sizeof(int) * M);
   return 0;
 }
 
@@ -539,17 +484,9 @@ extern "C" int svo_b200_depth_filter_update(svo_b200_ctx* ctx, const svo_b200_fr
   if (!ref_index || !ftr_px || !ftr_f || !ftr_level || !ftr_type || !ftr_grad || !batch_id || !a || !b || !mu ||
       !z_range || !sigma2 || !status_out)
     return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: NULL seed arrays");
-  for (int m = 0; m < M; ++m) {
-    if (ref_index[m] < 0 || ref_index[m] >= n_ref)
-      return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: ref_index[%d] out of range", m);
-    if (ftr_level[m] < 0 || ftr_level[m] >= ref_frames[ref_index[m]]->n_levels)
-      return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: ftr_level[%d] outside the pyramid", m);
-  }
-  if (opt->max_search_level >= cur->n_levels)
-    return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update: max_search_level %d >= %d pyramid levels",
-                   opt->max_search_level, cur->n_levels);
-  if (const int rc = cam_check_frames(ctx, "depth_filter_update", cam, &cur, 1)) return rc;
-  if (const int rc = cam_check_frames(ctx, "depth_filter_update", cam, ref_frames, n_ref)) return rc;
+  if (const int rc = check_ref_table(ctx, "depth_filter_update", "ftr_level", ref_frames, n_ref, M, ref_index, ftr_level, cur, cam,
+                                     opt->max_search_level))
+    return rc;
   DepthStream st;
   if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, batch_counter, st)) return rc;
   const int seed_offset[2] = {0, M};
@@ -591,12 +528,8 @@ extern "C" int svo_b200_depth_filter_update_streams(svo_b200_ctx* ctx, int S, co
     return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: NULL keyframe table or seed arrays");
   for (int r = 0; r < n_ref; ++r)
     if (!ref_frames[r]) return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: ref_frames[%d] is NULL", r);
-  for (int m = 0; m < M; ++m) {
-    if (ref_index[m] < 0 || ref_index[m] >= n_ref)
-      return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: ref_index[%d] out of range", m);
-    if (ftr_level[m] < 0 || ftr_level[m] >= ref_frames[ref_index[m]]->n_levels)
-      return set_err(ctx, SVO_B200_EINVAL, "depth_filter_update_streams: ftr_level[%d] outside the pyramid", m);
-  }
+  if (const int rc = check_ref_levels(ctx, "depth_filter_update_streams", "ftr_level", ref_frames, n_ref, M, ref_index, ftr_level))
+    return rc;
   // each stream's camera against its current frame and the keyframes its seeds refer to (the table is shared by streams
   // of different cameras)
   for (int s = 0; s < S; ++s) {
@@ -635,17 +568,9 @@ extern "C" int svo_b200_find_epipolar_match_direct(svo_b200_ctx* ctx, const svo_
   }
   if (!ref_index || !ftr_px || !ftr_f || !ftr_level || !ftr_type || !ftr_grad || !d_estimate || !d_min || !d_max || !success_out)
     return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: NULL candidate arrays");
-  for (int m = 0; m < M; ++m) {
-    if (ref_index[m] < 0 || ref_index[m] >= n_ref)
-      return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: ref_index[%d] out of range", m);
-    if (ftr_level[m] < 0 || ftr_level[m] >= ref_frames[ref_index[m]]->n_levels)
-      return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: ftr_level[%d] outside the pyramid", m);
-  }
-  if (opt->max_search_level >= cur->n_levels)
-    return set_err(ctx, SVO_B200_EINVAL, "find_epipolar_match_direct: max_search_level %d >= %d pyramid levels",
-                   opt->max_search_level, cur->n_levels);
-  if (const int rc = cam_check_frames(ctx, "find_epipolar_match_direct", cam, &cur, 1)) return rc;
-  if (const int rc = cam_check_frames(ctx, "find_epipolar_match_direct", cam, ref_frames, n_ref)) return rc;
+  if (const int rc = check_ref_table(ctx, "find_epipolar_match_direct", "ftr_level", ref_frames, n_ref, M, ref_index, ftr_level, cur, cam,
+                                     opt->max_search_level))
+    return rc;
   DepthStream st;
   if (const int rc = depth_stream(ctx, cur, cur_T_f_w, cam, 0, st)) return rc;
   const int seed_offset[2] = {0, M};

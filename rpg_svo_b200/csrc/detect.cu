@@ -183,11 +183,10 @@ int detect_check(svo_b200_ctx* ctx, const svo_b200_detect_stream& a) {
   return 0;
 }
 
-// One checked call: its table entry (device pointers filled in at staging), its grid and its CTA count.
+// One checked call: its table entry (device pointers set at staging), its grid and its CTA count.
 struct DetectCall {
   DetectStream t;
   int n_cells = 0, n_ctas = 0;
-  size_t o_cells = 0, o_occ = 0;
 };
 
 void detect_setup(const svo_b200_detect_stream& a, DetectCall& r) {
@@ -257,11 +256,7 @@ int detect_run(svo_b200_ctx* ctx, int S, const svo_b200_detect_stream* streams, 
   std::vector<DetectCall> calls((size_t)S);
   int64_t n_ctas = 0;
   for (int s = 0; s < S; ++s) {
-    if (const int rc = detect_check(ctx, streams[s])) {
-      if (!ctx || name == nullptr) return rc;
-      const std::string why = ctx->err;
-      return set_err(ctx, rc, "%s: stream %d: %s", name, s, why.c_str());
-    }
+    if (const int rc = detect_check(ctx, streams[s])) return entry_err(ctx, rc, name, "stream", s);
     detect_setup(streams[s], calls[s]);
     n_ctas += calls[s].n_ctas;
   }
@@ -269,44 +264,33 @@ int detect_run(svo_b200_ctx* ctx, int S, const svo_b200_detect_stream* streams, 
     return set_err(ctx, SVO_B200_ELIMIT, "fast_detect: %lld CTAs exceed one launch's grid", (long long)n_ctas);
   if (S == 0) return 0;
   cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_tab = c.take(sizeof(DetectStream) * S), o_off = c.take(sizeof(int) * (S + 1));
-  const size_t o_keys = c.take(0);  // every stream's cells back to back: one copy back
-  for (DetectCall& r : calls) r.o_cells = c.take(sizeof(unsigned long long) * r.n_cells, alignof(unsigned long long));
-  const size_t keys_end = c.off;
-  for (int s = 0; s < S; ++s) calls[s].o_occ = c.take(streams[s].grid_occupancy ? calls[s].n_cells : 0, 1);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  int* off = reinterpret_cast<int*>(h + o_off);
-  off[0] = 0;
+  std::vector<DetectStream> tab((size_t)S);
+  std::vector<int> cta_offset((size_t)S + 1, 0);
+  Staging st(ctx);
   for (int s = 0; s < S; ++s) {
-    DetectCall& r = calls[s];
-    const svo_b200_detect_stream& a = streams[s];
-    const unsigned long long init = detect_init_key(a.opt->detection_threshold);
-    unsigned long long* keys = reinterpret_cast<unsigned long long*>(h + r.o_cells);
-    for (int k = 0; k < r.n_cells; ++k) keys[k] = init;
-    if (a.grid_occupancy) std::memcpy(h + r.o_occ, a.grid_occupancy, r.n_cells);
-    r.t.occupancy = a.grid_occupancy ? d + r.o_occ : nullptr;
-    r.t.cells = reinterpret_cast<unsigned long long*>(d + r.o_cells);
-    reinterpret_cast<DetectStream*>(h + o_tab)[s] = r.t;
-    off[s + 1] = off[s] + r.n_ctas;
+    tab[s] = calls[s].t;
+    cta_offset[s + 1] = cta_offset[s] + calls[s].n_ctas;
+    if (streams[s].grid_occupancy) st.in(streams[s].grid_occupancy, calls[s].n_cells, &tab[s].occupancy, 1);
+    st.inout<unsigned long long>(nullptr, calls[s].n_cells, &tab[s].cells, alignof(unsigned long long));  // initial keys in
   }
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, c.off, cudaMemcpyHostToDevice, ctx->stream));
-  if (n_ctas > 0) {
-    kt_begin(ctx);
-    fast_detect_kernel<<<(unsigned)n_ctas, 256, 0, ctx->stream>>>(reinterpret_cast<const DetectStream*>(d + o_tab),
-                                                                   reinterpret_cast<const int*>(d + o_off), S);
-    ctx->launches++;
-    kt_end(ctx);
-    SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  const DetectStream* d_tab;
+  const int* d_off;
+  st.in(tab.data(), S, &d_tab);
+  st.in(cta_offset.data(), S + 1, &d_off);
+  int rc;
+  if ((rc = st.open())) return rc;
+  for (int s = 0; s < S; ++s) {
+    const unsigned long long init = detect_init_key(streams[s].opt->detection_threshold);
+    unsigned long long* keys = st.host(tab[s].cells);
+    for (int k = 0; k < calls[s].n_cells; ++k) keys[k] = init;
   }
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_keys, d + o_keys, keys_end - o_keys, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int s = 0; s < S; ++s) detect_decode(reinterpret_cast<const unsigned long long*>(h + calls[s].o_cells), calls[s], streams[s]);
+  if ((rc = st.send())) return rc;
+  if (n_ctas > 0 && (rc = launch_kernels(ctx, 1, [&] {
+        fast_detect_kernel<<<(unsigned)n_ctas, 256, 0, ctx->stream>>>(d_tab, d_off, S);
+      })))
+    return rc;
+  if ((rc = st.receive())) return rc;
+  for (int s = 0; s < S; ++s) detect_decode(st.host(tab[s].cells), calls[s], streams[s]);
   return 0;
 }
 

@@ -351,11 +351,7 @@ int klt_build_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds, co
   bool any_der = false;
   for (int s = 0; s < S; ++s) {
     KltBuild& r = bs[s];
-    if (const int rc = klt_build_check(ctx, builds[s], r.w, r.h, r.n)) {
-      if (!ctx || name == nullptr) return rc;
-      const std::string why = ctx->err;
-      return set_err(ctx, rc, "%s: build %d: %s", name, s, why.c_str());
-    }
+    if (const int rc = klt_build_check(ctx, builds[s], r.w, r.h, r.n)) return entry_err(ctx, rc, name, "build", s);
     for (int t = 0; t < s; ++t)
       if (builds[t].pyr == builds[s].pyr) return set_err(ctx, SVO_B200_EINVAL, "%s: builds %d and %d name one handle", name, t, s);
     Carver c;
@@ -429,18 +425,17 @@ int klt_build_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds, co
   }
   uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
   SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h.data(), c.off, cudaMemcpyHostToDevice, ctx->stream));
-  kt_begin(ctx);
-  const dim3 blk(32, 8);
-  for (int k = 0; k < n_launch; ++k) {
-    const KltJob* jobs = reinterpret_cast<const KltJob*>(d + o_jobs[k]);
-    const int* off = reinterpret_cast<const int*>(d + o_off[k]);
-    if (k == 0) klt_level0_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
-    else if (k < L_max) klt_down_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
-    else klt_scharr_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
-    ctx->launches++;
-  }
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  if ((rc = launch_kernels(ctx, n_launch, [&] {
+         const dim3 blk(32, 8);
+         for (int k = 0; k < n_launch; ++k) {
+           const KltJob* jobs = reinterpret_cast<const KltJob*>(d + o_jobs[k]);
+           const int* off = reinterpret_cast<const int*>(d + o_off[k]);
+           if (k == 0) klt_level0_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+           else if (k < L_max) klt_down_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+           else klt_scharr_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+         }
+       })))
+    return rc;
   for (int s = 0; s < S; ++s) {
     const KltBuild& r = bs[s];
     svo_b200_klt_pyramid* p = builds[s].pyr;
@@ -502,11 +497,7 @@ int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, 
   std::vector<KltStream> tab((size_t)S);
   int64_t n_pts = 0, n_ex = 0;
   for (int s = 0; s < S; ++s) {
-    if (const int rc = klt_track_check(ctx, streams[s])) {
-      if (!ctx || name == nullptr) return rc;
-      const std::string why = ctx->err;
-      return set_err(ctx, rc, "%s: stream %d: %s", name, s, why.c_str());
-    }
+    if (const int rc = klt_track_check(ctx, streams[s])) return entry_err(ctx, rc, name, "stream", s);
     tab[s] = klt_stream_entry(streams[s]);
     tab[s].pt_off = (int)std::min<int64_t>(n_pts, INT32_MAX);
     tab[s].ex_off = streams[s].exit_out ? (int)std::min<int64_t>(n_ex, INT32_MAX) : -1;
@@ -516,55 +507,47 @@ int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, 
   if (n_pts > INT32_MAX)
     return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld points exceed one launch", name ? name : "klt_track", (long long)n_pts);
   if (n_pts == 0) return 0;  // S == 0 included: no copy, no launch
-  const int N = (int)n_pts;
   cudaSetDevice(ctx->device);
-  Carver ci, co;
-  const size_t i_tab = ci.take(sizeof(KltStream) * S), i_off = ci.take(sizeof(int) * (S + 1));
-  const size_t i_prev = ci.take((size_t)N * 8), i_guess = ci.take((size_t)N * 8);
-  const size_t o_next = co.take((size_t)N * 8), o_st = co.take((size_t)N), o_ex = co.take((size_t)n_ex * sizeof(svo_b200_klt_exit));
+  std::vector<int> cta_offset((size_t)S + 1, 0);
+  for (int s = 0; s < S; ++s) cta_offset[s + 1] = cta_offset[s] + (streams[s].N + kWarps - 1) / kWarps;
+  Staging st(ctx);
+  const KltStream* d_tab;
+  const int* d_off;
+  const float2 *d_prev, *d_guess;
+  float2* d_next;
+  uint8_t* d_status;
+  svo_b200_klt_exit* d_ex;
+  st.in(tab.data(), S, &d_tab);
+  st.in(cta_offset.data(), S + 1, &d_off);
+  st.in(nullptr, n_pts, &d_prev);  // every stream's points and guesses, back to back
+  st.in(nullptr, n_pts, &d_guess);
+  st.out(nullptr, n_pts, &d_next);
+  st.out(nullptr, n_pts, &d_status);
+  st.out(nullptr, n_ex, &d_ex);
   int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, ci.off)) || (rc = ensure_dev(ctx, ctx->d_in, ci.off)) ||
-      (rc = ensure_host(ctx, ctx->h_out, co.off)) || (rc = ensure_dev(ctx, ctx->d_out, co.off)))
-    return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* hi = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* di = static_cast<uint8_t*>(ctx->d_in.p);
-  uint8_t* ho = static_cast<uint8_t*>(ctx->h_out.p);
-  uint8_t* dout = static_cast<uint8_t*>(ctx->d_out.p);
-  int* off = reinterpret_cast<int*>(hi + i_off);
-  off[0] = 0;
+  if ((rc = st.open())) return rc;
   for (int s = 0; s < S; ++s) {
     const svo_b200_klt_stream& a = streams[s];
-    reinterpret_cast<KltStream*>(hi + i_tab)[s] = tab[s];
-    off[s + 1] = off[s] + (a.N + kWarps - 1) / kWarps;
     if (a.N == 0) continue;
-    std::memcpy(hi + i_prev + (size_t)tab[s].pt_off * 8, a.prev_pts, (size_t)a.N * 8);
-    std::memcpy(hi + i_guess + (size_t)tab[s].pt_off * 8, a.next_pts_io, (size_t)a.N * 8);
+    std::memcpy(st.host(d_prev + tab[s].pt_off), a.prev_pts, (size_t)a.N * 8);
+    std::memcpy(st.host(d_guess + tab[s].pt_off), a.next_pts_io, (size_t)a.N * 8);
   }
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(di, hi, ci.off, cudaMemcpyHostToDevice, ctx->stream));
-  kt_begin(ctx);
-  const float2* d_prev = reinterpret_cast<const float2*>(di + i_prev);
-  const float2* d_guess = reinterpret_cast<const float2*>(di + i_guess);
-  float2* d_next = reinterpret_cast<float2*>(dout + o_next);
-  svo_b200_klt_exit* d_ex = reinterpret_cast<svo_b200_klt_exit*>(dout + o_ex);
-  if (S == 1)  // the table's entry by value (see klt_track_one_kernel); the staged table is then not read
-    klt_track_one_kernel<<<(unsigned)off[1], kWarps * 32, 0, ctx->stream>>>(tab[0], d_prev, d_guess, d_next, dout + o_st, d_ex);
-  else
-    klt_track_kernel<<<(unsigned)off[S], kWarps * 32, 0, ctx->stream>>>(reinterpret_cast<const KltStream*>(di + i_tab),
-                                                                         reinterpret_cast<const int*>(di + i_off), S, d_prev,
-                                                                         d_guess, d_next, dout + o_st, d_ex);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(ho, dout, co.off, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+  if ((rc = st.send())) return rc;
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         if (S == 1)  // the table's entry by value (see klt_track_one_kernel); the staged table is then not read
+           klt_track_one_kernel<<<(unsigned)cta_offset[1], kWarps * 32, 0, ctx->stream>>>(tab[0], d_prev, d_guess, d_next, d_status, d_ex);
+         else
+           klt_track_kernel<<<(unsigned)cta_offset[S], kWarps * 32, 0, ctx->stream>>>(d_tab, d_off, S, d_prev, d_guess, d_next, d_status,
+                                                                                     d_ex);
+       })))
+    return rc;
+  if ((rc = st.receive())) return rc;
   for (int s = 0; s < S; ++s) {
     const svo_b200_klt_stream& a = streams[s];
     if (a.N == 0) continue;
-    const size_t p = (size_t)tab[s].pt_off;
-    std::memcpy(a.next_pts_io, ho + o_next + p * 8, (size_t)a.N * 8);
-    std::memcpy(a.status_out, ho + o_st + p, (size_t)a.N);
-    if (a.exit_out) std::memcpy(a.exit_out, ho + o_ex + (size_t)tab[s].ex_off * sizeof(svo_b200_klt_exit), (size_t)a.N * sizeof(svo_b200_klt_exit));
+    std::memcpy(a.next_pts_io, st.host(d_next + tab[s].pt_off), (size_t)a.N * 8);
+    std::memcpy(a.status_out, st.host(d_status + tab[s].pt_off), (size_t)a.N);
+    if (a.exit_out) std::memcpy(a.exit_out, st.host(d_ex + tab[s].ex_off), (size_t)a.N * sizeof(svo_b200_klt_exit));
   }
   return 0;
 }

@@ -551,50 +551,25 @@ extern "C" int svo_b200_pose_optimize_batch(svo_b200_ctx* ctx, int B, double rep
   memset(out, 0, sizeof(*out) * (size_t)B);
   if (total == 0) return 0;  // errors.empty() -> return, for every frame
   cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_T = c.take(sizeof(double) * 12 * B), o_hp = c.take(total), o_out = c.take(sizeof(svo_b200_pose_opt_result) * B);
-  const size_t io_end = c.off;
-  const size_t o_f = c.take(sizeof(double) * 3 * total), o_pos = c.take(sizeof(double) * 3 * total),
-               o_lv = c.take(sizeof(int) * total), o_off = c.take(sizeof(int) * (B + 1)), o_fx = c.take(sizeof(double) * B);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_T, T_f_w_io, sizeof(double) * 12 * B);
-  memcpy(h + o_hp, has_point_io + base, total);
-  memset(h + o_out, 0, sizeof(svo_b200_pose_opt_result) * B);
-  memcpy(h + o_f, f + 3 * (size_t)base, sizeof(double) * 3 * total);
-  memcpy(h + o_pos, point_pos + 3 * (size_t)base, sizeof(double) * 3 * total);
-  memcpy(h + o_lv, level + base, sizeof(int) * total);
-  int* off = reinterpret_cast<int*>(h + o_off);
+  std::vector<int> off((size_t)B + 1);
   for (int b = 0; b <= B; ++b) off[b] = obs_offset[b] - base;
-  memcpy(h + o_fx, fx, sizeof(double) * B);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, c.off, cudaMemcpyHostToDevice, ctx->stream));
+  Staging st(ctx);
   PoseOptParams P;
-  P.f = reinterpret_cast<const double*>(d + o_f);
-  P.pos = reinterpret_cast<const double*>(d + o_pos);
-  P.level = reinterpret_cast<const int*>(d + o_lv);
-  P.has_point = d + o_hp;
-  P.obs_offset = reinterpret_cast<const int*>(d + o_off);
-  P.fx = reinterpret_cast<const double*>(d + o_fx);
+  st.in(f + 3 * (size_t)base, 3 * (size_t)total, &P.f);
+  st.in(point_pos + 3 * (size_t)base, 3 * (size_t)total, &P.pos);
+  st.in(level + base, total, &P.level);
+  st.in(off.data(), B + 1, &P.obs_offset);
+  st.in(fx, B, &P.fx);
+  st.inout(T_f_w_io, 12 * (size_t)B, &P.T_io);
+  st.inout(has_point_io + base, total, &P.has_point);
+  st.inout(out, B, &P.out);  // zeroed above
+  int rc;
+  if ((rc = st.open()) || (rc = st.send())) return rc;
   P.n_iter = n_iter;
   P.reproj_thresh = reproj_thresh;
-  P.T_io = reinterpret_cast<double*>(d + o_T);
-  P.out = reinterpret_cast<svo_b200_pose_opt_result*>(d + o_out);
   SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(pose_opt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kt_begin(ctx);
-  pose_opt_kernel<<<B, kPoThreads, smem, ctx->stream>>>(P);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h, d, io_end, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(T_f_w_io, h + o_T, sizeof(double) * 12 * B);
-  memcpy(has_point_io + base, h + o_hp, total);
-  memcpy(out, h + o_out, sizeof(*out) * (size_t)B);
-  return 0;
+  if ((rc = launch_kernels(ctx, 1, [&] { pose_opt_kernel<<<B, kPoThreads, smem, ctx->stream>>>(P); }))) return rc;
+  return st.receive();
 }
 
 extern "C" int svo_b200_pose_optimize(svo_b200_ctx* ctx, double reproj_thresh, int n_iter, double fx,
@@ -715,36 +690,23 @@ extern "C" int svo_b200_point_optimize_batch(svo_b200_ctx* ctx, int P, int n_ite
     if (obs_frame[obs_offset[0] + o] < 0 || obs_frame[obs_offset[0] + o] >= n_frames)
       return set_err(ctx, SVO_B200_EINVAL, "point_optimize_batch: obs_frame[%d] out of range", o);
   cudaSetDevice(ctx->device);
-  Carver c;
-  const size_t o_pos = c.take(sizeof(double) * 3 * P);
-  const size_t io_end = c.off;
-  const size_t o_off = c.take(sizeof(int) * (P + 1)), o_fr = c.take(sizeof(int) * (n_obs + 1)),
-               o_f = c.take(sizeof(double) * 3 * (n_obs + 1)), o_T = c.take(sizeof(double) * 12 * n_frames);
-  int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  memcpy(h + o_pos, pos_io, sizeof(double) * 3 * P);
-  int* off = reinterpret_cast<int*>(h + o_off);
+  std::vector<int> off((size_t)P + 1);
   for (int p = 0; p <= P; ++p) off[p] = obs_offset[p] - obs_offset[0];
-  memcpy(h + o_fr, obs_frame + obs_offset[0], sizeof(int) * n_obs);
-  memcpy(h + o_f, obs_f + 3 * (size_t)obs_offset[0], sizeof(double) * 3 * n_obs);
-  memcpy(h + o_T, frame_T_f_w, sizeof(double) * 12 * n_frames);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, c.off, cudaMemcpyHostToDevice, ctx->stream));
+  Staging st(ctx);
+  const int *d_off, *d_frame;
+  const double *d_f, *d_T;
+  double* d_pos;
+  st.in(off.data(), P + 1, &d_off);
+  st.in(obs_frame + obs_offset[0], n_obs, &d_frame);
+  st.in(obs_f + 3 * (size_t)obs_offset[0], 3 * (size_t)n_obs, &d_f);
+  st.in(frame_T_f_w, 12 * (size_t)n_frames, &d_T);
+  st.inout(pos_io, 3 * (size_t)P, &d_pos);
+  int rc;
+  if ((rc = st.open()) || (rc = st.send())) return rc;
   const int threads = 128, blocks = (P + threads - 1) / threads;
-  kt_begin(ctx);
-  point_optimize_kernel<<<blocks, threads, 0, ctx->stream>>>(P, n_iter, reinterpret_cast<const int*>(d + o_off),
-                                                             reinterpret_cast<const int*>(d + o_fr),
-                                                             reinterpret_cast<const double*>(d + o_f),
-                                                             reinterpret_cast<const double*>(d + o_T),
-                                                             reinterpret_cast<double*>(d + o_pos));
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_pos, d + o_pos, io_end - o_pos, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(pos_io, h + o_pos, sizeof(double) * 3 * P);
-  return 0;
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         point_optimize_kernel<<<blocks, threads, 0, ctx->stream>>>(P, n_iter, d_off, d_frame, d_f, d_T, d_pos);
+       })))
+    return rc;
+  return st.receive();
 }

@@ -267,58 +267,37 @@ void reproject_enumerate(ReprojCall& r) {
   for (int c = 0; c < m->n_candidates; ++c) { r.e_pt.push_back(m->cand_point[c]); r.e_src.push_back(-1); }
 }
 
-// Byte offsets of one call's device inputs and outputs in the context's staging buffer (mirrored host / device).
-struct ReprojLayout {
-  size_t o_ept, o_skip, o_pos, o_ooff, o_obs, o_fkf, o_fpx, o_ff, o_flv, o_fty, o_fgr, o_kT, o_kfr;
-  size_t o_px, o_in, o_cell, o_su, o_pm, o_sl, o_A, o_rf;
-};
-
-void reproject_carve_in(Carver& c, const svo_b200_map_view* m, int E, ReprojLayout& L) {
-  const int n_obs = m->n_points ? m->pt_obs_offset[m->n_points] : 0;
-  L.o_ept = c.take(sizeof(int) * E); L.o_skip = c.take(E); L.o_pos = c.take(sizeof(double) * 3 * m->n_points);
-  L.o_ooff = c.take(sizeof(int) * (m->n_points + 1)); L.o_obs = c.take(sizeof(int) * n_obs);
-  L.o_fkf = c.take(sizeof(int) * m->n_ftrs); L.o_fpx = c.take(sizeof(double) * 2 * m->n_ftrs);
-  L.o_ff = c.take(sizeof(double) * 3 * m->n_ftrs); L.o_flv = c.take(sizeof(int) * m->n_ftrs);
-  L.o_fty = c.take(sizeof(int) * m->n_ftrs); L.o_fgr = c.take(sizeof(double) * 2 * m->n_ftrs);
-  L.o_kT = c.take(sizeof(double) * 12 * m->n_kfs); L.o_kfr = c.take(sizeof(FrameDesc) * m->n_kfs);
-}
-
-void reproject_carve_out(Carver& c, int E, ReprojLayout& L) {
-  L.o_px = c.take(sizeof(double) * 2 * E); L.o_in = c.take(E); L.o_cell = c.take(sizeof(int) * E); L.o_su = c.take(E);
-  L.o_pm = c.take(sizeof(double) * 2 * E); L.o_sl = c.take(sizeof(int) * E); L.o_A = c.take(sizeof(double) * 4 * E);
-  L.o_rf = c.take(sizeof(int) * E);
-}
-
-// Stages one call's inputs into the host staging buffer h and fills its table entry with their device addresses (d).
-void reproject_stage(uint8_t* h, uint8_t* d, const ReprojLayout& L, const ReprojCall& r, ReprojStream& t) {
+// Declares one call's regions, their device addresses going into its table entry t: the map arrays and the enumeration
+// in (the skip flags and keyframe descriptors filled by reproject_run), the device results out.
+void reproject_stage(Staging& st, const ReprojCall& r, ReprojStream& t) {
   const svo_b200_map_view* m = r.a.map;
-  const int E = (int)r.e_pt.size(), n_obs = m->n_points ? m->pt_obs_offset[m->n_points] : 0;
-  auto cp = [&](size_t off, const void* src, size_t bytes) { if (bytes) memcpy(h + off, src, bytes); };  // empty tables may be NULL
-  cp(L.o_ept, r.e_pt.data(), sizeof(int) * E);
-  for (int e = 0; e < E; ++e) (h + L.o_skip)[e] = r.a.pt_type_io[r.e_pt[e]] == 0;
-  cp(L.o_pos, m->pt_pos, sizeof(double) * 3 * m->n_points);
-  cp(L.o_ooff, m->pt_obs_offset, sizeof(int) * (m->n_points + 1));
-  cp(L.o_obs, m->pt_obs, sizeof(int) * n_obs);
-  cp(L.o_fkf, m->ftr_kf, sizeof(int) * m->n_ftrs);
-  cp(L.o_fpx, m->ftr_px, sizeof(double) * 2 * m->n_ftrs);
-  cp(L.o_ff, m->ftr_f, sizeof(double) * 3 * m->n_ftrs);
-  cp(L.o_flv, m->ftr_level, sizeof(int) * m->n_ftrs);
-  cp(L.o_fty, m->ftr_type, sizeof(int) * m->n_ftrs);
-  cp(L.o_fgr, m->ftr_grad, sizeof(double) * 2 * m->n_ftrs);
-  cp(L.o_kT, m->kf_T_f_w, sizeof(double) * 12 * m->n_kfs);
-  for (int k = 0; k < m->n_kfs; ++k) reinterpret_cast<FrameDesc*>(h + L.o_kfr)[k] = make_desc(r.a.kf_frames[k]);
+  const size_t E = r.e_pt.size(), n_pts = m->n_points, n_ftrs = m->n_ftrs, n_kfs = m->n_kfs;
   memset(&t, 0, sizeof(t));
+  ReprojIn& in = t.in;
+  ReprojOut& out = t.out;
+  st.in(r.e_pt.data(), E, &in.e_pt);
+  st.in(nullptr, E, &in.e_skip);
+  st.in(m->pt_pos, 3 * n_pts, &in.pt_pos);
+  st.in(m->pt_obs_offset, n_pts + 1, &in.pt_obs_offset);
+  st.in(m->pt_obs, n_pts ? m->pt_obs_offset[n_pts] : 0, &in.pt_obs);
+  st.in(m->ftr_kf, n_ftrs, &in.ftr_kf);
+  st.in(m->ftr_px, 2 * n_ftrs, &in.ftr_px);
+  st.in(m->ftr_f, 3 * n_ftrs, &in.ftr_f);
+  st.in(m->ftr_level, n_ftrs, &in.ftr_level);
+  st.in(m->ftr_type, n_ftrs, &in.ftr_type);
+  st.in(m->ftr_grad, 2 * n_ftrs, &in.ftr_grad);
+  st.in(m->kf_T_f_w, 12 * n_kfs, &in.kf_T);
+  st.in(nullptr, n_kfs, &in.kf_frames);
+  st.out(nullptr, 2 * E, &out.px);
+  st.out(nullptr, E, &out.in_frame);
+  st.out(nullptr, E, &out.cell);
+  st.out(nullptr, E, &out.success);
+  st.out(nullptr, 2 * E, &out.px_match);
+  st.out(nullptr, E, &out.search_level);
+  st.out(nullptr, 4 * E, &out.A);
+  st.out(nullptr, E, &out.ref_ftr);
   t.cur = make_desc(r.a.cur);
   t.cam = r.cm;
-  t.in = {reinterpret_cast<const int*>(d + L.o_ept), d + L.o_skip, reinterpret_cast<const double*>(d + L.o_pos),
-          reinterpret_cast<const int*>(d + L.o_ooff), reinterpret_cast<const int*>(d + L.o_obs),
-          reinterpret_cast<const int*>(d + L.o_fkf), reinterpret_cast<const double*>(d + L.o_fpx),
-          reinterpret_cast<const double*>(d + L.o_ff), reinterpret_cast<const int*>(d + L.o_flv),
-          reinterpret_cast<const int*>(d + L.o_fty), reinterpret_cast<const double*>(d + L.o_fgr),
-          reinterpret_cast<const double*>(d + L.o_kT), reinterpret_cast<const FrameDesc*>(d + L.o_kfr)};
-  t.out = {reinterpret_cast<double*>(d + L.o_px), d + L.o_in, reinterpret_cast<int*>(d + L.o_cell), d + L.o_su,
-           reinterpret_cast<double*>(d + L.o_pm), reinterpret_cast<int*>(d + L.o_sl), reinterpret_cast<double*>(d + L.o_A),
-           reinterpret_cast<int*>(d + L.o_rf)};
   memcpy(t.cur_T_f_w, r.a.cur_T_f_w, sizeof(double) * 12);
   t.cell_size = r.a.opt->grid_size;
   t.grid_n_cols = r.grid_n_cols;
@@ -326,20 +305,15 @@ void reproject_stage(uint8_t* h, uint8_t* d, const ReprojLayout& L, const Reproj
   t.max_search_level = r.a.opt->max_search_level;
   t.align_max_iter = r.a.opt->align_max_iter;
 }
-// The host replay of the sequential policy over the device results of one call (in the host staging buffer h).
-void reproject_replay(const uint8_t* h, const ReprojLayout& L, const ReprojCall& r) {
+// The host replay of the sequential policy over the device results `o` of one call, in st's pinned buffer.
+void reproject_replay(const Staging& st, const ReprojOut& o, const ReprojCall& r) {
   const svo_b200_reproject_stream& a = r.a;
   const svo_b200_map_view* m = a.map;
   const svo_b200_reproject_options* opt = a.opt;
   const int E = (int)r.e_pt.size();
-  const double* r_px = reinterpret_cast<const double*>(h + L.o_px);
-  const uint8_t* r_in = h + L.o_in;
-  const int* r_cell = reinterpret_cast<const int*>(h + L.o_cell);
-  const uint8_t* r_su = h + L.o_su;
-  const double* r_pm = reinterpret_cast<const double*>(h + L.o_pm);
-  const int* r_sl = reinterpret_cast<const int*>(h + L.o_sl);
-  const double* r_A = reinterpret_cast<const double*>(h + L.o_A);
-  const int* r_rf = reinterpret_cast<const int*>(h + L.o_rf);
+  const double *r_px = st.host(o.px), *r_pm = st.host(o.px_match), *r_A = st.host(o.A);
+  const uint8_t *r_in = st.host(o.in_frame), *r_su = st.host(o.success);
+  const int *r_cell = st.host(o.cell), *r_sl = st.host(o.search_level), *r_rf = st.host(o.ref_ftr);
   std::vector<std::vector<int>> cells(r.n_cells);  // enumeration indices, push_back order
   for (int e = 0; e < E; ++e) {
     const int p = r.e_pt[e];
@@ -410,32 +384,30 @@ int reproject_run(svo_b200_ctx* ctx, const std::vector<ReprojCall>& calls) {
   const int A = (int)act.size(), E_total = e_offset.back();
   if (A == 0) return 0;
   cudaSetDevice(ctx->device);
-  Carver c;
-  std::vector<ReprojLayout> L((size_t)A);
-  for (int j = 0; j < A; ++j) reproject_carve_in(c, act[j]->a.map, (int)act[j]->e_pt.size(), L[j]);
-  const size_t o_tab = c.take(sizeof(ReprojStream) * A), o_off = c.take(sizeof(int) * (A + 1));
-  const size_t in_bytes = c.off;
-  for (int j = 0; j < A; ++j) reproject_carve_out(c, (int)act[j]->e_pt.size(), L[j]);
-  const size_t o_back = L[0].o_px;
+  Staging st(ctx);
+  std::vector<ReprojStream> tab((size_t)A);
+  for (int j = 0; j < A; ++j) reproject_stage(st, *act[j], tab[j]);
+  const ReprojStream* d_tab;
+  const int* d_off;
+  st.in(tab.data(), A, &d_tab);
+  st.in(e_offset.data(), A + 1, &d_off);
   int rc;
-  if ((rc = ensure_host(ctx, ctx->h_in, c.off))) return rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* h = static_cast<uint8_t*>(ctx->h_in.p);
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  for (int j = 0; j < A; ++j) reproject_stage(h, d, L[j], *act[j], reinterpret_cast<ReprojStream*>(h + o_tab)[j]);
-  memcpy(h + o_off, e_offset.data(), sizeof(int) * (A + 1));
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = st.open())) return rc;
+  for (int j = 0; j < A; ++j) {
+    const ReprojCall& r = *act[j];
+    uint8_t* skip = st.host(tab[j].in.e_skip);
+    for (size_t e = 0; e < r.e_pt.size(); ++e) skip[e] = r.a.pt_type_io[r.e_pt[e]] == 0;
+    FrameDesc* kfs = st.host(tab[j].in.kf_frames);
+    for (int k = 0; k < r.a.map->n_kfs; ++k) kfs[k] = make_desc(r.a.kf_frames[k]);
+  }
+  if ((rc = st.send())) return rc;
   const int blocks = (E_total + kRpWarps - 1) / kRpWarps;
-  kt_begin(ctx);
-  reproject_match_kernel<<<blocks, kRpWarps * 32, 0, ctx->stream>>>(reinterpret_cast<const ReprojStream*>(d + o_tab),
-                                                                     reinterpret_cast<const int*>(d + o_off), A, E_total);
-  ctx->launches++;
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(h + o_back, d + o_back, c.off - o_back, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int j = 0; j < A; ++j) reproject_replay(h, L[j], *act[j]);
+  if ((rc = launch_kernels(ctx, 1, [&] {
+         reproject_match_kernel<<<blocks, kRpWarps * 32, 0, ctx->stream>>>(d_tab, d_off, A, E_total);
+       })))
+    return rc;
+  if ((rc = st.receive())) return rc;
+  for (int j = 0; j < A; ++j) reproject_replay(st, tab[j].out, *act[j]);
   return 0;
 }
 
@@ -472,10 +444,7 @@ extern "C" int svo_b200_reproject_map_streams(svo_b200_ctx* ctx, int S, const sv
     r.a = streams[s];
     int rc = reproject_check(ctx, r.a);
     if (!rc) rc = reproject_grid(ctx, r);
-    if (rc) {
-      const std::string why = ctx->err;
-      return set_err(ctx, rc, "reproject_map_streams: stream %d: %s", s, why.c_str());
-    }
+    if (rc) return entry_err(ctx, rc, "reproject_map_streams", "stream", s);
     e_bound += (int64_t)(r.a.map->n_kfs ? r.a.map->kf_fts_offset[r.a.map->n_kfs] : 0) + r.a.map->n_candidates;
   }
   if (e_bound > INT32_MAX) return set_err(ctx, SVO_B200_ELIMIT, "reproject_map_streams: more than 2^31-1 points in one launch");
