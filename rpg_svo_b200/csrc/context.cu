@@ -76,7 +76,7 @@ int cam_check_frames(svo_b200_ctx* ctx, const char* who, const svo_b200_camera* 
   return 0;
 }
 
-int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes) {
+static int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes) {
   if (bytes <= b.cap) return 0;
   if (b.p) {
     SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
@@ -104,11 +104,11 @@ int Staging::open() {
   lay(false, true);
   end_ = c.off;
   int rc;
-  if ((rc = ensure_host(ctx_, ctx_->h_in, end_))) return rc;
-  if ((rc = ensure_dev(ctx_, ctx_->d_in, end_))) return rc;
+  if ((rc = ensure_host(ctx_, *hbuf_, end_))) return rc;
+  if ((rc = ensure_dev(ctx_, *dbuf_, end_))) return rc;
   SVO_CUDA_CHECK(ctx_, cudaStreamSynchronize(ctx_->stream));
-  h_ = static_cast<uint8_t*>(ctx_->h_in.p);
-  d_ = static_cast<uint8_t*>(ctx_->d_in.p);
+  h_ = static_cast<uint8_t*>(hbuf_->p);
+  d_ = static_cast<uint8_t*>(dbuf_->p);
   for (const Region& r : regions_) r.bind(r.at, d_ + r.off);
   for (const Region& r : regions_)
     if (r.in && r.src && r.bytes) memcpy(h_ + r.off, r.src, r.bytes);
@@ -714,7 +714,6 @@ void svo_b200_destroy(svo_b200_ctx* ctx) {
   sia_batch_free(ctx);
   sia_split_free(ctx);
   if (ctx->d_in.p) cudaFree(ctx->d_in.p);
-  if (ctx->d_scratch.p) cudaFree(ctx->d_scratch.p);
   if (ctx->h_in.p) cudaFreeHost(ctx->h_in.p);
   if (ctx->ev_k0) cudaEventDestroy(ctx->ev_k0);
   if (ctx->ev_k1) cudaEventDestroy(ctx->ev_k1);

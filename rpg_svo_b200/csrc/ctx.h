@@ -69,8 +69,8 @@ struct svo_b200_ctx {
   uint64_t launches = 0;
   int sm_count = 0;
   int max_smem_optin = 0;
-  // generic scratch: h_in / d_in hold an entry point's Staging, d_scratch the device-only arrays some carve
-  DevBuf d_in, d_scratch;
+  // generic scratch: h_in / d_in hold an entry point's Staging (the alignment batch has a pair of its own, SiaBatchState)
+  DevBuf d_in;
   HostBuf h_in;
   svo::SiaBatchState* sia = nullptr;
   cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around the kernel(s) of the last entry point (svo_b200_last_kernel_ms)
@@ -109,7 +109,6 @@ namespace svo {
 
 int set_err(svo_b200_ctx* ctx, int code, const char* fmt, ...);
 int ensure_dev(svo_b200_ctx* ctx, DevBuf& b, size_t bytes);
-int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes);
 
 #define SVO_CUDA_CHECK(ctx, call)                                                                   \
   do {                                                                                              \
@@ -153,8 +152,9 @@ int launch_kernels(svo_b200_ctx* ctx, int n, F&& launch) {
   return 0;
 }
 
-// An entry point's arrays staged through the context's pinned buffer and its device mirror (h_in / d_in).  Each region is
-// declared once, by kind, element count and the pointer `at` that open() sets to its device address:
+// An entry point's arrays staged through a pinned buffer and its device mirror: the context's h_in / d_in, or a pair of the
+// caller's own (the alignment batch's).  Each region is declared once, by kind, element count and the pointer `at` that
+// open() sets to its device address:
 //   in     copied in from src; a NULL src is filled by the caller through host() between open() and send();
 //   inout  copied in from io and back to it; a NULL io is filled and read by the caller;
 //   out    copied back to dst; a NULL dst is read by the caller through host(), or by nobody.
@@ -170,7 +170,8 @@ class Staging {
   using same_t = typename same<T>::type;  // element types come from `at` alone
 
  public:
-  explicit Staging(svo_b200_ctx* ctx) : ctx_(ctx) {}
+  explicit Staging(svo_b200_ctx* ctx) : Staging(ctx, ctx->h_in, ctx->d_in) {}
+  Staging(svo_b200_ctx* ctx, HostBuf& h, DevBuf& d) : ctx_(ctx), hbuf_(&h), dbuf_(&d) {}
   template <class T>
   void in(const same_t<T>* src, size_t n, T** at, size_t align = 256) { add(src, nullptr, sizeof(T) * n, align, true, false, at); }
   template <class T>
@@ -201,6 +202,8 @@ class Staging {
     regions_.push_back({src, dst, bytes, align, 0, in, back, at, [](void* a, uint8_t* p) { *static_cast<T**>(a) = reinterpret_cast<T*>(p); }});
   }
   svo_b200_ctx* ctx_;
+  HostBuf* hbuf_;
+  DevBuf* dbuf_;
   std::vector<Region> regions_;
   uint8_t *h_ = nullptr, *d_ = nullptr;
   size_t front_ = 0, back_ = 0, end_ = 0;

@@ -2052,31 +2052,29 @@ struct SiaBatchState {
   int total_feat = 0;
   int max_feat = 0;
   SiaParams P;
-  size_t in_bytes = 0;
   // The batch API owns its staging buffers: stage / run / fetch may be interleaved with any other entry point of the
-  // context (align, pose optimizer, depth filter ... reuse the context's generic scratch) without clobbering a staged
-  // batch.
-  DevBuf d_in, d_out;
-  HostBuf h_in, h_out;
-  size_t o_T = 0, o_H = 0, o_vis = 0, o_stats = 0, out_bytes = 0;
+  // context (align, pose optimizer, depth filter ... stage through the context's h_in / d_in) without clobbering a staged
+  // batch.  `io` is the Staging of the last stage, over this pair; it bound the addresses in P and `scales`.
+  HostBuf h;
+  DevBuf d;
+  Staging io;
   const SiaEntry* geo = nullptr;  // the launch geometry pick_launch chose (nullptr: the robust kernel)
   size_t smem = 0;
   bool staged = false;
   // robust cost (svo_b200_sia_robust) the batch was staged with: weight function, or -1 = unweighted (sia_kernel)
   int robust_weight = -1;
   int robust_slots = 0;
-  size_t o_scales = 0;
+  float* scales = nullptr;  // the robust kernel's per-pair, per-level scales (device)
   // features whose xyz_ref is not finite (sia_kernel only): staged without their point, visibility as the reference has it
   struct Nonfinite { int feat, pair, vis_levels; };  // vis_levels: the levels the set-only mask holds it at
   std::vector<Nonfinite> nonfinite;
+  explicit SiaBatchState(svo_b200_ctx* ctx) : io(ctx, h, d) {}
 };
 
 void sia_batch_free(svo_b200_ctx* ctx) {
   if (ctx->sia) {
-    if (ctx->sia->d_in.p) cudaFree(ctx->sia->d_in.p);
-    if (ctx->sia->d_out.p) cudaFree(ctx->sia->d_out.p);
-    if (ctx->sia->h_in.p) cudaFreeHost(ctx->sia->h_in.p);
-    if (ctx->sia->h_out.p) cudaFreeHost(ctx->sia->h_out.p);
+    if (ctx->sia->d.p) cudaFree(ctx->sia->d.p);
+    if (ctx->sia->h.p) cudaFreeHost(ctx->sia->h.p);
   }
   delete ctx->sia;
   ctx->sia = nullptr;
@@ -2254,13 +2252,9 @@ static int launch_sia_robust(svo_b200_ctx* ctx, const SiaBatchState& st) {
   RP.P = st.P;
   RP.weight = st.robust_weight;
   RP.slots = st.robust_slots;
-  RP.scales_out = reinterpret_cast<float*>(static_cast<uint8_t*>(st.d_out.p) + st.o_scales);
+  RP.scales_out = st.scales;
   SVO_CUDA_CHECK(ctx, cudaFuncSetAttribute(sia_robust_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.smem));
-  kt_begin(ctx);
-  sia_robust_kernel<<<st.B, kSiaRobustThreads, st.smem, ctx->stream>>>(RP);
-  kt_end(ctx);
-  ctx->launches++;
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
+  if (int rc = launch_kernels(ctx, 1, [&] { sia_robust_kernel<<<st.B, kSiaRobustThreads, st.smem, ctx->stream>>>(RP); })) return rc;
   svo_b200_sia_launch& L = ctx->sia_last;
   L = svo_b200_sia_launch{};
   L.n_pairs = st.B; L.ctas_per_pair = 1; L.threads = kSiaRobustThreads;
@@ -2464,14 +2458,16 @@ int svo_b200_sia_last_launch(const svo_b200_ctx* ctx, svo_b200_sia_launch* out) 
 
 namespace svo {
 // svo_b200_sia_batch_stage with the robust cost of the context (`robust`) or without it (svo_b200_sparse_residuals).
+// `more(st)` declares the extra regions of a single-pair call in st.io, after every check and before it opens.
+template <class More>
 static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref, const svo_b200_frame* const* cur,
                      const svo_b200_camera* cam, const svo_b200_sia_options* opt, const double* T, const int* feat_offset,
                      const double* px, const double* f, const double* point_pos, const uint8_t* has_point, const double* ref_pos,
-                     bool robust) {
+                     bool robust, More&& more) {
   if (!ctx || B <= 0 || !ref || !cur || !cam || !opt || !T || !feat_offset || !ref_pos)
     return set_err(ctx, SVO_B200_EINVAL, "sia_batch_stage: bad arguments");
   cudaSetDevice(ctx->device);
-  if (!ctx->sia) ctx->sia = new SiaBatchState();
+  if (!ctx->sia) ctx->sia = new SiaBatchState(ctx);
   SiaBatchState& st = *ctx->sia;
   st.staged = false;
   ctx->sia_chain = false;
@@ -2512,22 +2508,24 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
     if (rc) return rc;
   }
 
-  // input staging: [jobs B][blobs]
-  Carver cin;
-  const size_t o_jobs = cin.take(sizeof(SiaJob) * (size_t)B);
-  std::vector<size_t> o_blob(B);
-  for (int b = 0; b < B; ++b) {
-    const int n = feat_offset[b + 1] - feat_offset[b];
-    o_blob[b] = cin.take((size_t)pad16(n) * 65 + 16, 128);
-  }
-  st.in_bytes = cin.off;
-  if ((rc = ensure_host(ctx, st.h_in, st.in_bytes))) return rc;
-  if ((rc = ensure_dev(ctx, st.d_in, st.in_bytes))) return rc;
-  // a previous async copy out of the pinned buffer must be finished before it is rewritten
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  uint8_t* hin = static_cast<uint8_t*>(st.h_in.p);
-  uint8_t* din = static_cast<uint8_t*>(st.d_in.p);
-  SiaJob* jobs = reinterpret_cast<SiaJob*>(hin + o_jobs);
+  // in: the jobs, then the pairs' feature blobs, each on a 128-byte boundary (the jobs hold the blobs' addresses: both are
+  // filled after open()); out: read back by svo_b200_sia_batch_fetch
+  const auto blob_span = [](int n) { return ((size_t)pad16(n) * 65 + 16 + 127) / 128 * 128; };
+  size_t blob_bytes = 0;
+  for (int b = 0; b < B; ++b) blob_bytes += blob_span(feat_offset[b + 1] - feat_offset[b]);
+  st.io = Staging(ctx, st.h, st.d);
+  st.io.in(nullptr, B, &st.P.jobs);
+  const uint8_t* blobs = nullptr;
+  st.io.in(nullptr, blob_bytes, &blobs, 128);
+  st.io.out(nullptr, 12 * (size_t)B, &st.P.T_out);
+  st.io.out(nullptr, 36 * (size_t)B, &st.P.H_out);
+  st.io.out(nullptr, B, &st.P.stats);
+  st.io.out(nullptr, (size_t)st.total_feat + 16, &st.P.visible_out);
+  if (weighted) st.io.out(nullptr, SVO_B200_MAX_LEVELS * (size_t)B, &st.scales);
+  more(st);
+  if ((rc = st.io.open())) return rc;
+  SiaJob* jobs = st.io.host(st.P.jobs);
+  const uint8_t* blob = blobs;
   for (int b = 0; b < B; ++b) {
     SiaJob& j = jobs[b];
     memset(&j, 0, sizeof(j));
@@ -2539,41 +2537,26 @@ static int sia_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* const* ref,
     j.n_feat = n;
     j.n_pad = pad16(n);
     j.feat_off = o - feat_offset[0];
-    j.blob = din + o_blob[b];
+    j.blob = blob;
+    blob += blob_span(n);
     memcpy(j.T, T + 12 * (size_t)b, sizeof(double) * 12);
     memcpy(j.ref_pos, ref_pos + 3 * (size_t)b, sizeof(double) * 3);
-    if (n > 0) pack_blob(hin + o_blob[b], n, j.n_pad, px + 2 * (size_t)o, f + 3 * (size_t)o,
-                         point_pos + 3 * (size_t)o, has_point + o);
+    uint8_t* hb = st.io.host(j.blob);
+    if (n > 0) pack_blob(hb, n, j.n_pad, px + 2 * (size_t)o, f + 3 * (size_t)o, point_pos + 3 * (size_t)o, has_point + o);
     if (!weighted)
       for (int i = 0; i < n; ++i)
         if (has_point[o + i] && !finite_xyz_ref(f + 3 * (size_t)(o + i), point_pos + 3 * (size_t)(o + i), ref_pos + 3 * (size_t)b)) {
-          double* d = reinterpret_cast<double*>(hin + o_blob[b]);
+          double* d = reinterpret_cast<double*>(hb);
           const double* rp = ref_pos + 3 * (size_t)b;
           for (int c = 0; c < 3; ++c) {  // the neutral xyz_ref (0, 0, ~1) of a slot without a feature
             d[2 * (size_t)j.n_pad + 3 * i + c] = c == 2 ? 1.0 : 0.0;
             d[5 * (size_t)j.n_pad + 3 * i + c] = c == 2 ? rp[c] + 1.0 : rp[c];
           }
-          hin[o_blob[b] + (size_t)j.n_pad * 64 + i] = 0;
+          hb[(size_t)j.n_pad * 64 + i] = 0;
           st.nonfinite.push_back({j.feat_off + i, b, ref_patch_levels(px + 2 * (size_t)(o + i), st.P, ref[b])});
         }
   }
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(din, hin, st.in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-
-  Carver co;
-  st.o_T = co.take(sizeof(double) * 12 * (size_t)B);
-  st.o_H = co.take(sizeof(double) * 36 * (size_t)B);
-  st.o_stats = co.take(sizeof(svo_b200_sia_stats) * (size_t)B);
-  st.o_vis = co.take((size_t)st.total_feat + 16);
-  if (weighted) st.o_scales = co.take(sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)B);
-  st.out_bytes = co.off;
-  if ((rc = ensure_dev(ctx, st.d_out, st.out_bytes))) return rc;
-  if ((rc = ensure_host(ctx, st.h_out, st.out_bytes))) return rc;
-  uint8_t* dout = static_cast<uint8_t*>(st.d_out.p);
-  st.P.jobs = reinterpret_cast<const SiaJob*>(din + o_jobs);
-  st.P.T_out = reinterpret_cast<double*>(dout + st.o_T);
-  st.P.H_out = reinterpret_cast<double*>(dout + st.o_H);
-  st.P.stats = reinterpret_cast<svo_b200_sia_stats*>(dout + st.o_stats);
-  st.P.visible_out = dout + st.o_vis;
+  if ((rc = st.io.send())) return rc;
   st.staged = true;
   return 0;
 }
@@ -2586,7 +2569,7 @@ int svo_b200_sia_batch_stage(svo_b200_ctx* ctx, int B, const svo_b200_frame* con
                              const svo_b200_sia_options* opt, const double* T, const int* feat_offset,
                              const double* px, const double* f, const double* point_pos,
                              const uint8_t* has_point, const double* ref_pos) {
-  return sia_stage(ctx, B, ref, cur, cam, opt, T, feat_offset, px, f, point_pos, has_point, ref_pos, true);
+  return sia_stage(ctx, B, ref, cur, cam, opt, T, feat_offset, px, f, point_pos, has_point, ref_pos, true, [](SiaBatchState&) {});
 }
 
 int svo_b200_sia_batch_run(svo_b200_ctx* ctx) {
@@ -2604,20 +2587,18 @@ int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_
   cudaSetDevice(ctx->device);
   SiaBatchState& st = *ctx->sia;
   ctx->sia_chain = false;
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(st.h_out.p, st.d_out.p, st.out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ctx->xg_connected) {  // did every peer take part in every exchange?
+  if (int rc = st.io.receive()) return rc;
+  if (ctx->xg_connected) {  // did every peer take part in every exchange?  (if not, no caller array is written)
     std::vector<unsigned> err((size_t)st.B, 0u);
     SVO_CUDA_CHECK(ctx, cudaMemcpy2D(err.data(), sizeof(unsigned), static_cast<const uint8_t*>(ctx->xg_buf) + offsetof(XgPair, err),
                                      sizeof(XgPair), sizeof(unsigned), (size_t)st.B, cudaMemcpyDeviceToHost));
     for (int b = 0; b < st.B; ++b)
       if (err[b]) return set_err(ctx, SVO_B200_ECUDA, "sia split: a peer rank did not arrive at an exchange of pair %d (timeout); reconnect the split", b);
   }
-  const uint8_t* h = static_cast<const uint8_t*>(st.h_out.p);
-  if (T_out) memcpy(T_out, h + st.o_T, sizeof(double) * 12 * (size_t)st.B);
-  if (H_out) memcpy(H_out, h + st.o_H, sizeof(double) * 36 * (size_t)st.B);
-  if (stats_out) memcpy(stats_out, h + st.o_stats, sizeof(svo_b200_sia_stats) * (size_t)st.B);
-  if (visible_out) memcpy(visible_out, h + st.o_vis, (size_t)st.total_feat);
+  if (T_out) memcpy(T_out, st.io.host(st.P.T_out), sizeof(double) * 12 * (size_t)st.B);
+  if (H_out) memcpy(H_out, st.io.host(st.P.H_out), sizeof(double) * 36 * (size_t)st.B);
+  if (stats_out) memcpy(stats_out, st.io.host(st.P.stats), sizeof(svo_b200_sia_stats) * (size_t)st.B);
+  if (visible_out) memcpy(visible_out, st.io.host(st.P.visible_out), (size_t)st.total_feat);
   if (st.P.n_iter == 0 && st.robust_weight < 0) {
     // no iteration: SparseImgAlign computes the reference patches, and so the visibility, only inside the first residual
     // pass (the robust cost's scale pass at the start pose computes them there): no feature is visible at any level
@@ -2631,7 +2612,7 @@ int svo_b200_sia_batch_fetch(svo_b200_ctx* ctx, double* T_out, uint8_t* visible_
     }
   }
   if (st.robust_weight >= 0 && ctx->sia_last_robust && ctx->sia_scales.size() == (size_t)st.B * SVO_B200_MAX_LEVELS)
-    memcpy(ctx->sia_scales.data(), h + st.o_scales, sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)st.B);
+    memcpy(ctx->sia_scales.data(), st.io.host(st.scales), sizeof(float) * SVO_B200_MAX_LEVELS * (size_t)st.B);
   return 0;
 }
 
@@ -2649,36 +2630,25 @@ int svo_b200_sparse_img_align(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
     if (n_trace_out) *n_trace_out = 0;
     return 0;
   }
+  const bool tracing = trace_out && trace_cap > 0;
   const int off[2] = {0, N};
-  int rc = svo_b200_sia_batch_stage(ctx, 1, &ref, &cur, cam, opt, T_io, off, px, f, point_pos, has_point, ref_pos);
+  int rc = sia_stage(ctx, 1, &ref, &cur, cam, opt, T_io, off, px, f, point_pos, has_point, ref_pos, true, [&](SiaBatchState& st) {
+    if (!tracing) return;
+    st.io.out(nullptr, (size_t)trace_cap, &st.P.trace);
+    st.io.out(nullptr, 1, &st.P.n_trace);
+    st.P.trace_cap = trace_cap;
+  });
   if (rc) return rc;
   SiaBatchState& st = *ctx->sia;
-  size_t o_tr = 0, o_ntr = 0;
-  if (trace_out && trace_cap > 0) {
-    Carver c;
-    o_tr = c.take(sizeof(svo_b200_sia_iter) * (size_t)trace_cap);
-    o_ntr = c.take(sizeof(int));
-    if ((rc = ensure_dev(ctx, ctx->d_scratch, c.off))) return rc;
-    uint8_t* ds = static_cast<uint8_t*>(ctx->d_scratch.p);
-    st.P.trace = reinterpret_cast<svo_b200_sia_iter*>(ds + o_tr);
-    st.P.trace_cap = trace_cap;
-    st.P.n_trace = reinterpret_cast<int*>(ds + o_ntr);
-  }
   if ((rc = svo_b200_sia_batch_run(ctx))) return rc;
   if ((rc = svo_b200_sia_batch_fetch(ctx, T_io, visible_out, H_out, stats_out))) return rc;
-  if (trace_out && trace_cap > 0) {
-    int ntr = 0;
-    uint8_t* ds = static_cast<uint8_t*>(ctx->d_scratch.p);
-    SVO_CUDA_CHECK(ctx, cudaMemcpy(&ntr, ds + o_ntr, sizeof(int), cudaMemcpyDeviceToHost));
+  int ntr = 0;
+  if (tracing) {
+    ntr = *st.io.host(st.P.n_trace);
     const int ncopy = ntr < trace_cap ? ntr : trace_cap;
-    if (ncopy > 0)
-      SVO_CUDA_CHECK(ctx, cudaMemcpy(trace_out, ds + o_tr, sizeof(svo_b200_sia_iter) * (size_t)ncopy, cudaMemcpyDeviceToHost));
-    if (n_trace_out) *n_trace_out = ntr;
-  } else if (n_trace_out) {
-    *n_trace_out = 0;
+    if (ncopy > 0) memcpy(trace_out, st.io.host(st.P.trace), sizeof(svo_b200_sia_iter) * (size_t)ncopy);
   }
-  st.P.trace = nullptr;
-  st.P.n_trace = nullptr;
+  if (n_trace_out) *n_trace_out = ntr;
   st.staged = false;  // the single-pair call leaves nothing staged behind
   return 0;
 }
@@ -2693,39 +2663,31 @@ int svo_b200_sparse_residuals(svo_b200_ctx* ctx, const svo_b200_frame* ref, cons
     return set_err(ctx, SVO_B200_EINVAL, "sparse_residuals: bad arguments");
   svo_b200_sia_options opt = {level, level, 1, 1e-6};
   const int off[2] = {0, N};
-  int rc = sia_stage(ctx, 1, &ref, &cur, cam, &opt, T, off, px, f, point_pos, has_point, ref_pos, false);  // never weighted
+  size_t nslots = 0;  // feature slots of the launch geometry: the kernel writes a patch row of each
+  const auto regions = [&](SiaBatchState& st) {
+    nslots = (size_t)st.geo->threads * st.geo->fpt * st.geo->cluster;
+    st.io.in(visible_io, N, &st.P.visible_in);
+    st.io.out(nullptr, 16 * nslots, &st.P.ref_patch_out);
+    st.io.out(nullptr, 16 * nslots, &st.P.residuals_out);
+    st.io.out(nullptr, N, &st.P.in_image_out);
+    st.io.out(nullptr, 6, &st.P.Jres_out);
+    st.io.out(nullptr, 1, &st.P.chi2_out);
+    st.io.out(nullptr, 1, &st.P.n_meas_out);
+  };
+  int rc = sia_stage(ctx, 1, &ref, &cur, cam, &opt, T, off, px, f, point_pos, has_point, ref_pos, false, regions);  // never weighted
   if (rc) return rc;
   SiaBatchState& st = *ctx->sia;
-  const size_t nslots = (size_t)st.geo->threads * st.geo->fpt * st.geo->cluster;
-  Carver c;
-  const size_t o_vin = c.take(N), o_rp = c.take(sizeof(float) * 16 * nslots),
-               o_res = c.take(sizeof(float) * 16 * nslots), o_in = c.take(N),
-               o_j = c.take(sizeof(double) * 6), o_c = c.take(sizeof(double)), o_n = c.take(sizeof(long long));
-  if ((rc = ensure_dev(ctx, ctx->d_scratch, c.off))) return rc;
-  uint8_t* ds = static_cast<uint8_t*>(ctx->d_scratch.p);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(ds + o_vin, visible_io, N, cudaMemcpyHostToDevice, ctx->stream));
-  SVO_CUDA_CHECK(ctx, cudaMemsetAsync(ds + o_res, 0xff, sizeof(float) * 16 * nslots, ctx->stream));
+  SVO_CUDA_CHECK(ctx, cudaMemsetAsync(st.P.residuals_out, 0xff, sizeof(float) * 16 * nslots, ctx->stream));
   st.P.eval_level = level;
-  st.P.visible_in = ds + o_vin;
-  st.P.ref_patch_out = reinterpret_cast<float*>(ds + o_rp);
-  st.P.residuals_out = reinterpret_cast<float*>(ds + o_res);
-  st.P.in_image_out = ds + o_in;
-  st.P.Jres_out = reinterpret_cast<double*>(ds + o_j);
-  st.P.chi2_out = reinterpret_cast<double*>(ds + o_c);
-  st.P.n_meas_out = reinterpret_cast<long long*>(ds + o_n);
   if ((rc = launch_sia(ctx, st.P, 1, *st.geo, st.smem, true, false))) return rc;
   double Tdummy[12];
   if ((rc = svo_b200_sia_batch_fetch(ctx, Tdummy, visible_io, H_out, nullptr))) return rc;
-  if (ref_patch_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(ref_patch_out, ds + o_rp, sizeof(float) * 16 * (size_t)N, cudaMemcpyDeviceToHost));
-  if (residuals_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(residuals_out, ds + o_res, sizeof(float) * 16 * (size_t)N, cudaMemcpyDeviceToHost));
-  if (in_image_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(in_image_out, ds + o_in, N, cudaMemcpyDeviceToHost));
-  if (Jres_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(Jres_out, ds + o_j, sizeof(double) * 6, cudaMemcpyDeviceToHost));
-  if (chi2_out) SVO_CUDA_CHECK(ctx, cudaMemcpy(chi2_out, ds + o_c, sizeof(double), cudaMemcpyDeviceToHost));
-  if (n_meas_out) {
-    long long nm = 0;
-    SVO_CUDA_CHECK(ctx, cudaMemcpy(&nm, ds + o_n, sizeof(long long), cudaMemcpyDeviceToHost));
-    *n_meas_out = nm;
-  }
+  if (ref_patch_out) memcpy(ref_patch_out, st.io.host(st.P.ref_patch_out), sizeof(float) * 16 * (size_t)N);
+  if (residuals_out) memcpy(residuals_out, st.io.host(st.P.residuals_out), sizeof(float) * 16 * (size_t)N);
+  if (in_image_out) memcpy(in_image_out, st.io.host(st.P.in_image_out), N);
+  if (Jres_out) memcpy(Jres_out, st.io.host(st.P.Jres_out), sizeof(double) * 6);
+  if (chi2_out) *chi2_out = *st.io.host(st.P.chi2_out);
+  if (n_meas_out) *n_meas_out = *st.io.host(st.P.n_meas_out);
   st.staged = false;
   return 0;
 }
