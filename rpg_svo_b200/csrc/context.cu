@@ -91,6 +91,9 @@ static int ensure_host(svo_b200_ctx* ctx, HostBuf& b, size_t bytes) {
 }
 
 int Staging::open() {
+  if (!hbuf_)
+    for (const Region& r : regions_)
+      if (r.back) return set_err(ctx_, SVO_B200_EINVAL, "Staging: a pageable staging copies nothing back");
   Carver c;
   const auto lay = [&](bool in, bool back) {
     for (Region& r : regions_)
@@ -104,10 +107,15 @@ int Staging::open() {
   lay(false, true);
   end_ = c.off;
   int rc;
-  if ((rc = ensure_host(ctx_, *hbuf_, end_))) return rc;
+  if (hbuf_ && (rc = ensure_host(ctx_, *hbuf_, end_))) return rc;
   if ((rc = ensure_dev(ctx_, *dbuf_, end_))) return rc;
-  SVO_CUDA_CHECK(ctx_, cudaStreamSynchronize(ctx_->stream));
-  h_ = static_cast<uint8_t*>(hbuf_->p);
+  if (hbuf_) {
+    SVO_CUDA_CHECK(ctx_, cudaStreamSynchronize(ctx_->stream));
+    h_ = static_cast<uint8_t*>(hbuf_->p);
+  } else {
+    page_.resize(end_);
+    h_ = page_.data();
+  }
   d_ = static_cast<uint8_t*>(dbuf_->p);
   for (const Region& r : regions_) r.bind(r.at, d_ + r.off);
   for (const Region& r : regions_)
@@ -422,9 +430,8 @@ __global__ void __launch_bounds__(256) tile_levels_table_kernel(const PyrJob* __
   tile_block(jb.src, jb.w, jb.h, jb.tiled, b);
 }
 
-// tile_levels_kernel over levels [from, to) of frames [first, first + count) of `pool`
-static int tile_levels(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int first, int count, int from, int to) {
-  if (from >= to) return 0;
+// The tile_levels_kernel launch over levels [from, to) of frames [first, first + count) of `pool`
+static void tile_levels(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int first, int count, int from, int to) {
   const svo_b200_frame& f = pool->frames[first];
   TileGeom g;
   memset(&g, 0, sizeof(g));
@@ -436,9 +443,6 @@ static int tile_levels(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int f
   long long blocks = (n + 255) / 256;
   if (blocks > ctx->sm_count * 8LL) blocks = ctx->sm_count * 8LL;
   tile_levels_kernel<<<dim3((unsigned)blocks, (unsigned)(to - from)), 256, 0, ctx->stream>>>(g, from, count);
-  ctx->launches++;
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  return 0;
 }
 
 // does producing a level from a source level of width `src_w` use vikit's SSE2 rounding?  (x86 rule: width % 16 == 0;
@@ -484,53 +488,25 @@ static UploadPlan upload_plan(const svo_b200_frame& f, int n_given) {
 static int build_pyramid(svo_b200_ctx* ctx, const svo_b200_frame_pool* pool, int first, int count, int n_given) {
   const svo_b200_frame& f0 = pool->frames[0];
   const int n_levels = f0.n_levels;
-  kt_begin(ctx);
   const UploadPlan p = upload_plan(f0, n_given);
-  if (p.l0_l1) {
-    pyramid_l0_l1_stream_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(pool->slab[0], pool->stride[0], pool->slab[1],
-                                                                            pool->stride[1], pool->tslab[0], pool->tstride[0],
-                                                                            first, count, f0.w[0], f0.h[0], pyr_avg(ctx, f0.w[0]));
-    ctx->launches++;
-  }
-  if (int rc = tile_levels(ctx, pool, first, count, p.tile_from, p.tile_to)) return rc;
-  for (int top = p.top; top + 1 < n_levels; top += 4) {  // the fused kernel's level 0 = our level `top`
-    const PyrGeom g = pass_geom(ctx, f0, top, pool->stride, pool->tstride);
-    const int tiles_y = (g.h[0] + 15) / 16;
-    for (int done = 0; done < count; done += 32768) {  // gridDim.y limit 65535
-      const int n = count - done < 32768 ? count - done : 32768;
-      pyramid_fused_kernel<<<dim3(g.tiles_x * tiles_y, n), 128, 0, ctx->stream>>>(first + done, g);
-      ctx->launches++;
+  const int passes = (n_levels + 2 - p.top) / 4;  // top = p.top, p.top + 4, ... while top + 1 < n_levels
+  const int chunks = (count + 32767) / 32768;     // gridDim.y limit 65535
+  return launch_kernels(ctx, p.l0_l1 + (p.tile_from < p.tile_to) + passes * chunks, [&] {
+    if (p.l0_l1)
+      pyramid_l0_l1_stream_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(pool->slab[0], pool->stride[0], pool->slab[1],
+                                                                              pool->stride[1], pool->tslab[0], pool->tstride[0],
+                                                                              first, count, f0.w[0], f0.h[0], pyr_avg(ctx, f0.w[0]));
+    if (p.tile_from < p.tile_to) tile_levels(ctx, pool, first, count, p.tile_from, p.tile_to);
+    for (int top = p.top; top + 1 < n_levels; top += 4) {  // the fused kernel's level 0 = our level `top`
+      const PyrGeom g = pass_geom(ctx, f0, top, pool->stride, pool->tstride);
+      const int tiles_y = (g.h[0] + 15) / 16;
+      for (int done = 0; done < count; done += 32768) {
+        const int n = count - done < 32768 ? count - done : 32768;
+        pyramid_fused_kernel<<<dim3(g.tiles_x * tiles_y, n), 128, 0, ctx->stream>>>(first + done, g);
+      }
     }
-  }
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  kt_end(ctx);
-  return 0;
+  });
 }
-
-// The entries of one table-driven launch and the CTA offsets stream_of searches, with where the call's staging buffer
-// holds them.
-template <class Job>
-struct LaunchTable {
-  std::vector<Job> jobs;
-  std::vector<int> cta_offset = {0};
-  long long ctas = 0;
-  bool over = false;  // more CTAs than one grid holds, or a job whose thread index leaves int
-  size_t o_jobs = 0, o_off = 0;
-  void add(const Job& j, long long items, int per_cta) {
-    ctas += (items + per_cta - 1) / per_cta;
-    over = over || ctas > INT32_MAX || items > INT32_MAX - per_cta;
-    jobs.push_back(j);
-    cta_offset.push_back((int)std::min<long long>(ctas, INT32_MAX));
-  }
-  void carve(Carver& c) {
-    o_jobs = c.take(sizeof(Job) * jobs.size());
-    o_off = c.take(sizeof(int) * cta_offset.size());
-  }
-  void fill(uint8_t* h) const {
-    memcpy(h + o_jobs, jobs.data(), sizeof(Job) * jobs.size());
-    memcpy(h + o_off, cta_offset.data(), sizeof(int) * cta_offset.size());
-  }
-};
 
 // svo_b200_frame_upload(ctx, entries[s].frame, &entries[s].level0, 1) of every entry, with one launch per stage: every
 // entry is checked before anything is copied or launched; then each level 0 is copied into its frame, the tables of every
@@ -569,41 +545,23 @@ static int upload_streams(svo_b200_ctx* ctx, int S, const svo_b200_frame_upload_
   for (const auto& t : passes) over = over || t.over;
   if (over) return set_err(ctx, SVO_B200_ELIMIT, "%s: a launch's work exceeds one grid", who);
   if (S == 0) return 0;
-  Carver c;
-  l0_l1.carve(c);
-  tile.carve(c);
-  for (auto& t : passes) t.carve(c);
+  Staging st(ctx, Staging::Pageable{});
+  l0_l1.stage(st);
+  tile.stage(st);
+  for (auto& t : passes) t.stage(st);
   cudaSetDevice(ctx->device);
-  if (int rc = ensure_dev(ctx, ctx->d_in, c.off)) return rc;
-  std::vector<uint8_t> h(c.off);  // pageable: the copy stages it before returning, so no wait on earlier work
-  l0_l1.fill(h.data());
-  tile.fill(h.data());
-  for (const auto& t : passes) t.fill(h.data());
+  int rc;
+  if ((rc = st.open())) return rc;
   for (int s = 0; s < S; ++s) {
     const svo_b200_frame& f = *entries[s].frame;
     SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(f.lv[0], entries[s].level0, (size_t)f.w[0] * f.h[0], cudaMemcpyHostToDevice, ctx->stream));
   }
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h.data(), c.off, cudaMemcpyHostToDevice, ctx->stream));
-  kt_begin(ctx);
-  auto jobs = [&](const LaunchTable<PyrJob>& t) { return reinterpret_cast<const PyrJob*>(d + t.o_jobs); };
-  auto offs = [&](size_t o) { return reinterpret_cast<const int*>(d + o); };
-  if (!l0_l1.jobs.empty()) {
-    pyramid_l0_l1_table_kernel<<<(unsigned)l0_l1.ctas, 256, 0, ctx->stream>>>(jobs(l0_l1), offs(l0_l1.o_off), (int)l0_l1.jobs.size());
-    ctx->launches++;
-  }
-  if (!tile.jobs.empty()) {
-    tile_levels_table_kernel<<<(unsigned)tile.ctas, 256, 0, ctx->stream>>>(jobs(tile), offs(tile.o_off), (int)tile.jobs.size());
-    ctx->launches++;
-  }
-  for (const auto& t : passes) {
-    pyramid_fused_table_kernel<<<(unsigned)t.ctas, 128, 0, ctx->stream>>>(reinterpret_cast<const PyrGeom*>(d + t.o_jobs), offs(t.o_off),
-                                                                         (int)t.jobs.size());
-    ctx->launches++;
-  }
-  kt_end(ctx);
-  SVO_CUDA_CHECK(ctx, cudaGetLastError());
-  return 0;
+  if ((rc = st.send())) return rc;
+  return launch_kernels(ctx, (l0_l1.n() > 0) + (tile.n() > 0) + (int)passes.size(), [&] {
+    if (l0_l1.n()) pyramid_l0_l1_table_kernel<<<(unsigned)l0_l1.ctas, 256, 0, ctx->stream>>>(l0_l1.jobs_at, l0_l1.off_at, l0_l1.n());
+    if (tile.n()) tile_levels_table_kernel<<<(unsigned)tile.ctas, 256, 0, ctx->stream>>>(tile.jobs_at, tile.off_at, tile.n());
+    for (const auto& t : passes) pyramid_fused_table_kernel<<<(unsigned)t.ctas, 128, 0, ctx->stream>>>(t.jobs_at, t.off_at, t.n());
+  });
 }
 
 // A zeroed pool of `count` frames of one geometry (arguments checked by the caller); `who` prefixes the error messages.

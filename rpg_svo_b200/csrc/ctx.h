@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -163,6 +164,10 @@ int launch_kernels(svo_b200_ctx* ctx, int n, F&& launch) {
 // buffer), sets every `at` and then copies the sources in, so that a table whose entries hold region addresses can itself
 // be a source.  send() copies the front range to the device; receive() copies the tail range back, waits for it and
 // copies every region with a destination out.
+// The pageable form (Staging(ctx, Staging::Pageable{})) stages in-only regions into d_in through a host buffer of its own,
+// made per call.  The runtime stages a copy from pageable memory before the copy returns, so open() does not wait for the
+// stream (only growing d_in does), and a call that only copies in does not wait on earlier work.  open() refuses in-out and
+// out regions.
 class Staging {
   template <class T>
   struct same { using type = T; };
@@ -170,8 +175,10 @@ class Staging {
   using same_t = typename same<T>::type;  // element types come from `at` alone
 
  public:
+  struct Pageable {};
   explicit Staging(svo_b200_ctx* ctx) : Staging(ctx, ctx->h_in, ctx->d_in) {}
   Staging(svo_b200_ctx* ctx, HostBuf& h, DevBuf& d) : ctx_(ctx), hbuf_(&h), dbuf_(&d) {}
+  Staging(svo_b200_ctx* ctx, Pageable) : ctx_(ctx), hbuf_(nullptr), dbuf_(&ctx->d_in) {}
   template <class T>
   void in(const same_t<T>* src, size_t n, T** at, size_t align = 256) { add(src, nullptr, sizeof(T) * n, align, true, false, at); }
   template <class T>
@@ -202,11 +209,38 @@ class Staging {
     regions_.push_back({src, dst, bytes, align, 0, in, back, at, [](void* a, uint8_t* p) { *static_cast<T**>(a) = reinterpret_cast<T*>(p); }});
   }
   svo_b200_ctx* ctx_;
-  HostBuf* hbuf_;
+  HostBuf* hbuf_;  // NULL: pageable, through page_
   DevBuf* dbuf_;
+  std::vector<uint8_t> page_;
   std::vector<Region> regions_;
   uint8_t *h_ = nullptr, *d_ = nullptr;
   size_t front_ = 0, back_ = 0, end_ = 0;
+};
+
+// The entries of one table-driven launch, where a CTA finds its entry with stream_of over the CTA offsets: entry j holds
+// `items` work items, `per_cta` to a CTA, and CTAs cta_offset[j] .. cta_offset[j + 1] - 1.  stage() declares the entries
+// and the offsets as two in-regions of `st`, whose device addresses open() sets in `jobs_at` / `off_at`.  An entry that
+// holds region addresses is added before any region binding into it is declared, so that `jobs` never reallocates under a
+// bound pointer.
+template <class Job>
+struct LaunchTable {
+  std::vector<Job> jobs;
+  std::vector<int> cta_offset = {0};
+  long long ctas = 0;
+  bool over = false;  // more CTAs than one grid holds, or an entry whose thread index leaves int
+  const Job* jobs_at = nullptr;
+  const int* off_at = nullptr;
+  void add(const Job& j, long long items, int per_cta) {
+    ctas += (items + per_cta - 1) / per_cta;
+    over = over || ctas > INT32_MAX || items > INT32_MAX - per_cta;
+    jobs.push_back(j);
+    cta_offset.push_back((int)std::min<long long>(ctas, INT32_MAX));
+  }
+  int n() const { return (int)jobs.size(); }
+  void stage(Staging& st) {
+    st.in(jobs.data(), jobs.size(), &jobs_at);
+    st.in(cta_offset.data(), cta_offset.size(), &off_at);
+  }
 };
 
 // Re-prefixes the error that the check of entry i of a many-entry call left: "<name>: <what> <i>: <message>".  A single

@@ -254,43 +254,35 @@ void detect_decode(const unsigned long long* keys, const DetectCall& r, const sv
 // occupancy grids), one launch, one copy back of all cells, and each stream's decode into its own outputs.
 int detect_run(svo_b200_ctx* ctx, int S, const svo_b200_detect_stream* streams, const char* name) {
   std::vector<DetectCall> calls((size_t)S);
-  int64_t n_ctas = 0;
+  LaunchTable<DetectStream> tab;
   for (int s = 0; s < S; ++s) {
     if (const int rc = detect_check(ctx, streams[s])) return entry_err(ctx, rc, name, "stream", s);
     detect_setup(streams[s], calls[s]);
-    n_ctas += calls[s].n_ctas;
+    tab.add(calls[s].t, calls[s].n_ctas, 1);
   }
-  if (n_ctas > INT32_MAX)
-    return set_err(ctx, SVO_B200_ELIMIT, "fast_detect: %lld CTAs exceed one launch's grid", (long long)n_ctas);
+  if (tab.over) return set_err(ctx, SVO_B200_ELIMIT, "fast_detect: %lld CTAs exceed one launch's grid", tab.ctas);
   if (S == 0) return 0;
   cudaSetDevice(ctx->device);
-  std::vector<DetectStream> tab((size_t)S);
-  std::vector<int> cta_offset((size_t)S + 1, 0);
   Staging st(ctx);
   for (int s = 0; s < S; ++s) {
-    tab[s] = calls[s].t;
-    cta_offset[s + 1] = cta_offset[s] + calls[s].n_ctas;
-    if (streams[s].grid_occupancy) st.in(streams[s].grid_occupancy, calls[s].n_cells, &tab[s].occupancy, 1);
-    st.inout<unsigned long long>(nullptr, calls[s].n_cells, &tab[s].cells, alignof(unsigned long long));  // initial keys in
+    if (streams[s].grid_occupancy) st.in(streams[s].grid_occupancy, calls[s].n_cells, &tab.jobs[s].occupancy, 1);
+    st.inout<unsigned long long>(nullptr, calls[s].n_cells, &tab.jobs[s].cells, alignof(unsigned long long));  // initial keys in
   }
-  const DetectStream* d_tab;
-  const int* d_off;
-  st.in(tab.data(), S, &d_tab);
-  st.in(cta_offset.data(), S + 1, &d_off);
+  tab.stage(st);
   int rc;
   if ((rc = st.open())) return rc;
   for (int s = 0; s < S; ++s) {
     const unsigned long long init = detect_init_key(streams[s].opt->detection_threshold);
-    unsigned long long* keys = st.host(tab[s].cells);
+    unsigned long long* keys = st.host(tab.jobs[s].cells);
     for (int k = 0; k < calls[s].n_cells; ++k) keys[k] = init;
   }
   if ((rc = st.send())) return rc;
-  if (n_ctas > 0 && (rc = launch_kernels(ctx, 1, [&] {
-        fast_detect_kernel<<<(unsigned)n_ctas, 256, 0, ctx->stream>>>(d_tab, d_off, S);
+  if (tab.ctas > 0 && (rc = launch_kernels(ctx, 1, [&] {
+        fast_detect_kernel<<<(unsigned)tab.ctas, 256, 0, ctx->stream>>>(tab.jobs_at, tab.off_at, S);
       })))
     return rc;
   if ((rc = st.receive())) return rc;
-  for (int s = 0; s < S; ++s) detect_decode(st.host(tab[s].cells), calls[s], streams[s]);
+  for (int s = 0; s < S; ++s) detect_decode(st.host(tab.jobs[s].cells), calls[s], streams[s]);
   return 0;
 }
 

@@ -361,32 +361,26 @@ int klt_build_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds, co
     L_max = std::max(L_max, r.n);
     any_der = any_der || builds[s].with_derivatives;
   }
-  // jobs of every launch, back to back: level 0, levels 1 .. L_max - 1, Scharr
+  // one table per launch: level 0, levels 1 .. L_max - 1, Scharr; the jobs' addresses are set once the blocks are allocated
   const int n_launch = L_max + (any_der ? 1 : 0);
-  std::vector<int> n_jobs((size_t)n_launch, 0);
-  std::vector<int64_t> n_ctas((size_t)n_launch, 0);
+  std::vector<LaunchTable<KltJob>> tabs((size_t)n_launch);
   for (int s = 0; s < S; ++s) {
     const KltBuild& r = bs[s];
     for (int l = 0; l < r.n; ++l) {
-      n_jobs[l]++;
-      n_ctas[l] += tiles(r.w[l], r.h[l]);
-      if (builds[s].with_derivatives) { n_jobs[L_max]++; n_ctas[L_max] += tiles(r.w[l], r.h[l]); }
+      const int64_t n = tiles(r.w[l], r.h[l]);
+      tabs[l].add(KltJob{nullptr, nullptr, nullptr, l == 0 ? r.w[0] : r.w[l - 1], r.w[l], r.h[l], tiles_x(r.w[l])}, n, 1);
+      if (builds[s].with_derivatives) tabs[L_max].add(KltJob{nullptr, nullptr, nullptr, r.w[l], r.w[l], r.h[l], tiles_x(r.w[l])}, n, 1);
     }
   }
-  for (int k = 0; k < n_launch; ++k)
-    if (n_ctas[k] > INT32_MAX)
-      return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld CTAs exceed one launch's grid", name ? name : "klt_pyramid_build",
-                     (long long)n_ctas[k]);
+  for (const auto& t : tabs)
+    if (t.over)
+      return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld CTAs exceed one launch's grid", name ? name : "klt_pyramid_build", t.ctas);
   if (S == 0) return 0;
-  Carver c;
-  std::vector<size_t> o_jobs((size_t)n_launch), o_off((size_t)n_launch);
-  for (int k = 0; k < n_launch; ++k) {
-    o_jobs[k] = c.take(sizeof(KltJob) * n_jobs[k]);
-    o_off[k] = c.take(sizeof(int) * (n_jobs[k] + 1));
-  }
+  Staging st(ctx, Staging::Pageable{});
+  for (auto& t : tabs) t.stage(st);
   cudaSetDevice(ctx->device);
   int rc;
-  if ((rc = ensure_dev(ctx, ctx->d_in, c.off))) return rc;
+  if ((rc = st.open())) return rc;
   for (int s = 0; s < S; ++s) {
     svo_b200_klt_pyramid* p = builds[s].pyr;
     if (bs[s].bytes <= p->bytes) continue;
@@ -404,35 +398,29 @@ int klt_build_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_build* builds, co
     }
     p->bytes = bs[s].bytes;
   }
-  std::vector<uint8_t> h(c.off);  // pageable: the copy stages it before returning, so no wait on earlier work
-  std::vector<int> fill((size_t)n_launch, 0);
-  for (int k = 0; k < n_launch; ++k) reinterpret_cast<int*>(h.data() + o_off[k])[0] = 0;
-  auto add = [&](int k, const KltJob& j) {
-    reinterpret_cast<KltJob*>(h.data() + o_jobs[k])[fill[k]] = j;
-    int* off = reinterpret_cast<int*>(h.data() + o_off[k]);
-    off[fill[k] + 1] = off[fill[k]] + (int)tiles(j.w, j.h);
-    fill[k]++;
-  };
+  std::vector<int> next((size_t)n_launch, 0);  // jobs of each table addressed so far, in the order they were added
   for (int s = 0; s < S; ++s) {
     const KltBuild& r = bs[s];
     uint8_t* base = static_cast<uint8_t*>(builds[s].pyr->mem);
     for (int l = 0; l < r.n; ++l) {
-      const uint8_t* src = l == 0 ? builds[s].frame->lvl(0) : base + r.off[l - 1];
-      add(l, KltJob{src, base + r.off[l], nullptr, l == 0 ? r.w[0] : r.w[l - 1], r.w[l], r.h[l], tiles_x(r.w[l])});
-      if (builds[s].with_derivatives)
-        add(L_max, KltJob{base + r.off[l], nullptr, reinterpret_cast<int*>(base + r.doff[l]), r.w[l], r.w[l], r.h[l], tiles_x(r.w[l])});
+      KltJob& j = st.host(tabs[l].jobs_at)[next[l]++];
+      j.src = l == 0 ? builds[s].frame->lvl(0) : base + r.off[l - 1];
+      j.dst = base + r.off[l];
+      if (builds[s].with_derivatives) {
+        KltJob& d = st.host(tabs[L_max].jobs_at)[next[L_max]++];
+        d.src = base + r.off[l];
+        d.der = reinterpret_cast<int*>(base + r.doff[l]);
+      }
     }
   }
-  uint8_t* d = static_cast<uint8_t*>(ctx->d_in.p);
-  SVO_CUDA_CHECK(ctx, cudaMemcpyAsync(d, h.data(), c.off, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = st.send())) return rc;
   if ((rc = launch_kernels(ctx, n_launch, [&] {
          const dim3 blk(32, 8);
          for (int k = 0; k < n_launch; ++k) {
-           const KltJob* jobs = reinterpret_cast<const KltJob*>(d + o_jobs[k]);
-           const int* off = reinterpret_cast<const int*>(d + o_off[k]);
-           if (k == 0) klt_level0_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
-           else if (k < L_max) klt_down_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
-           else klt_scharr_kernel<<<(unsigned)n_ctas[k], blk, 0, ctx->stream>>>(jobs, off, n_jobs[k]);
+           const LaunchTable<KltJob>& t = tabs[k];
+           if (k == 0) klt_level0_kernel<<<(unsigned)t.ctas, blk, 0, ctx->stream>>>(t.jobs_at, t.off_at, t.n());
+           else if (k < L_max) klt_down_kernel<<<(unsigned)t.ctas, blk, 0, ctx->stream>>>(t.jobs_at, t.off_at, t.n());
+           else klt_scharr_kernel<<<(unsigned)t.ctas, blk, 0, ctx->stream>>>(t.jobs_at, t.off_at, t.n());
          }
        })))
     return rc;
@@ -494,13 +482,14 @@ KltStream klt_stream_entry(const svo_b200_klt_stream& a) {
 // points and guesses), one launch, one copy back of every stream's points, statuses and exit records, and each stream's
 // share copied into its own outputs.
 int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, const char* name) {
-  std::vector<KltStream> tab((size_t)S);
+  LaunchTable<KltStream> tab;
   int64_t n_pts = 0, n_ex = 0;
   for (int s = 0; s < S; ++s) {
     if (const int rc = klt_track_check(ctx, streams[s])) return entry_err(ctx, rc, name, "stream", s);
-    tab[s] = klt_stream_entry(streams[s]);
-    tab[s].pt_off = (int)std::min<int64_t>(n_pts, INT32_MAX);
-    tab[s].ex_off = streams[s].exit_out ? (int)std::min<int64_t>(n_ex, INT32_MAX) : -1;
+    KltStream e = klt_stream_entry(streams[s]);
+    e.pt_off = (int)std::min<int64_t>(n_pts, INT32_MAX);
+    e.ex_off = streams[s].exit_out ? (int)std::min<int64_t>(n_ex, INT32_MAX) : -1;
+    tab.add(e, streams[s].N, kWarps);
     n_pts += streams[s].N;
     if (streams[s].exit_out) n_ex += streams[s].N;
   }
@@ -508,17 +497,12 @@ int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, 
     return set_err(ctx, SVO_B200_ELIMIT, "%s: %lld points exceed one launch", name ? name : "klt_track", (long long)n_pts);
   if (n_pts == 0) return 0;  // S == 0 included: no copy, no launch
   cudaSetDevice(ctx->device);
-  std::vector<int> cta_offset((size_t)S + 1, 0);
-  for (int s = 0; s < S; ++s) cta_offset[s + 1] = cta_offset[s] + (streams[s].N + kWarps - 1) / kWarps;
   Staging st(ctx);
-  const KltStream* d_tab;
-  const int* d_off;
   const float2 *d_prev, *d_guess;
   float2* d_next;
   uint8_t* d_status;
   svo_b200_klt_exit* d_ex;
-  st.in(tab.data(), S, &d_tab);
-  st.in(cta_offset.data(), S + 1, &d_off);
+  tab.stage(st);
   st.in(nullptr, n_pts, &d_prev);  // every stream's points and guesses, back to back
   st.in(nullptr, n_pts, &d_guess);
   st.out(nullptr, n_pts, &d_next);
@@ -529,25 +513,25 @@ int klt_track_run(svo_b200_ctx* ctx, int S, const svo_b200_klt_stream* streams, 
   for (int s = 0; s < S; ++s) {
     const svo_b200_klt_stream& a = streams[s];
     if (a.N == 0) continue;
-    std::memcpy(st.host(d_prev + tab[s].pt_off), a.prev_pts, (size_t)a.N * 8);
-    std::memcpy(st.host(d_guess + tab[s].pt_off), a.next_pts_io, (size_t)a.N * 8);
+    std::memcpy(st.host(d_prev + tab.jobs[s].pt_off), a.prev_pts, (size_t)a.N * 8);
+    std::memcpy(st.host(d_guess + tab.jobs[s].pt_off), a.next_pts_io, (size_t)a.N * 8);
   }
   if ((rc = st.send())) return rc;
   if ((rc = launch_kernels(ctx, 1, [&] {
          if (S == 1)  // the table's entry by value (see klt_track_one_kernel); the staged table is then not read
-           klt_track_one_kernel<<<(unsigned)cta_offset[1], kWarps * 32, 0, ctx->stream>>>(tab[0], d_prev, d_guess, d_next, d_status, d_ex);
+           klt_track_one_kernel<<<(unsigned)tab.ctas, kWarps * 32, 0, ctx->stream>>>(tab.jobs[0], d_prev, d_guess, d_next, d_status, d_ex);
          else
-           klt_track_kernel<<<(unsigned)cta_offset[S], kWarps * 32, 0, ctx->stream>>>(d_tab, d_off, S, d_prev, d_guess, d_next, d_status,
-                                                                                     d_ex);
+           klt_track_kernel<<<(unsigned)tab.ctas, kWarps * 32, 0, ctx->stream>>>(tab.jobs_at, tab.off_at, S, d_prev, d_guess, d_next,
+                                                                                d_status, d_ex);
        })))
     return rc;
   if ((rc = st.receive())) return rc;
   for (int s = 0; s < S; ++s) {
     const svo_b200_klt_stream& a = streams[s];
     if (a.N == 0) continue;
-    std::memcpy(a.next_pts_io, st.host(d_next + tab[s].pt_off), (size_t)a.N * 8);
-    std::memcpy(a.status_out, st.host(d_status + tab[s].pt_off), (size_t)a.N);
-    if (a.exit_out) std::memcpy(a.exit_out, st.host(d_ex + tab[s].ex_off), (size_t)a.N * sizeof(svo_b200_klt_exit));
+    std::memcpy(a.next_pts_io, st.host(d_next + tab.jobs[s].pt_off), (size_t)a.N * 8);
+    std::memcpy(a.status_out, st.host(d_status + tab.jobs[s].pt_off), (size_t)a.N);
+    if (a.exit_out) std::memcpy(a.exit_out, st.host(d_ex + tab.jobs[s].ex_off), (size_t)a.N * sizeof(svo_b200_klt_exit));
   }
   return 0;
 }
